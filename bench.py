@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""bench.py - MVS depth-pixels/second of the dmrecon hot path on B200 (BASELINE.json metric).
+"""bench.py - MVS depth-pixels/second of the dmrecon hot path on H100 (BASELINE.json metric).
 
     python bench.py --gpus N --steps K --warmup W            # our arm (one rank per GPU under torchrun for N > 1)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's own CPU dmrecon on the host cores
     python bench.py --workload C3|C4|C5 --gpus N ...         # the other BASELINE configs (nominally 8 / 4 / 8 GPUs)
+    python bench.py ... --dump-outputs DIR                   # also write the maps of the last timed step as DIR/*.npy
 
 Workload (default, N = 1): BASELINE.json configs[1] (C2) - synthetic 16-view 1920x1080 scene, dmrecon scale = 1, all 16
 views reconstructed; one step = DMRecon::start for all 16 reference views.  N > 1: the same per-GPU work (16 reference
@@ -73,7 +74,7 @@ def workload_text(name, scene):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -226,6 +227,30 @@ def reference_arm(args, real_stdout):
 # ----------------------------------------------------------------------------------------------------------------
 # our arm
 # ----------------------------------------------------------------------------------------------------------------
+DUMP_BYTES_MAX = 64 << 20
+
+
+def dump_outputs(out_dir, maps, rank, world):
+    """The maps the caller of the last timed end-to-end step received (one dict of depth / conf / dz per reference view
+    of this rank), stacked over views as <out_dir>/{depth,conf,dz}.npy (suffix _rank<r> when world > 1).  Above 64 MB in
+    all, every view is reduced to the same seeded sample of pixels, whose flat indices go to pixel_index.npy (float64).
+    The bench inputs are seeded, so two builds run with the same arguments can be compared file by file."""
+    os.makedirs(out_dir, exist_ok=True)
+    sfx = "_rank%d" % rank if world > 1 else ""
+    H, W = maps[0]["depth"].shape
+    per_px = sum(a.itemsize * (a.size // (H * W)) for a in maps[0].values()) * len(maps)
+    n_px = min(H * W, (DUMP_BYTES_MAX - 4096) // world // (per_px + 8))       # 4 KB for the .npy headers
+    idx = None
+    if n_px < H * W:
+        idx = np.sort(np.random.default_rng(0).choice(H * W, size=n_px, replace=False))
+        np.save(os.path.join(out_dir, "pixel_index%s.npy" % sfx), idx.astype(np.float64))
+    for k in ("depth", "conf", "dz"):
+        a = np.stack([np.asarray(m[k], np.float32).reshape(H * W, -1) for m in maps])
+        if idx is not None:
+            a = a[:, idx]
+        np.save(os.path.join(out_dir, "%s%s.npy" % (k, sfx)), a.reshape(a.shape[:2]) if k != "dz" else a)
+
+
 def _protect_stdout():
     """Everything but the one JSON line goes to stderr: libraries (NCCL prints its version banner on stdout) must not
     pollute the line the driver parses.  Returns a file object bound to the original stdout."""
@@ -252,6 +277,8 @@ def _main(real_stdout):
     ap.add_argument("--workload", default="C2")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--cpu-seconds", type=float, default=15.0)
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the depth / conf / dz maps of the last timed end-to-end step "
+                                                          "as DIR/<name>.npy (float32; a seeded pixel sample if > 64 MB)")
     args = ap.parse_args()
     args.steps = max(1, args.steps)
     args.warmup = max(0, args.warmup)
@@ -326,7 +353,7 @@ def _main(real_stdout):
         out_bufs.append(dict(depth=torch.empty((Hs, Ws), dtype=torch.float32).pin_memory().numpy(),
                              conf=torch.empty((Hs, Ws), dtype=torch.float32).pin_memory().numpy(),
                              dz=torch.empty((Hs, Ws, 2), dtype=torch.float32).pin_memory().numpy()))
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)      # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)      # > 50 MB L2
 
     def barrier():
         torch.cuda.synchronize()
@@ -405,6 +432,8 @@ def _main(real_stdout):
     barrier()
     e2e_elapsed = time.perf_counter() - t0
     f_e2e_total, _ = agg(f_e2e)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, out_bufs, rank, world)
     _, e2e_max = agg(e2e_elapsed)
     h2d = int(host_imgs.numel())
     d2h = int(sum(b["depth"].nbytes + b["conf"].nbytes + b["dz"].nbytes for b in out_bufs))
@@ -412,13 +441,8 @@ def _main(real_stdout):
     planner.shutdown()
 
     # ---- roofline of the dominant kernel (k_frontier: the persistent kernel that runs every PatchOptimization), rank 0 ----
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6.65 TB/s (B200_PROFILING.md)"
+    peak = 3350.0
+    peak_src = "H100 SXM data sheet, 3.35 TB/s HBM3 (not measured)"
     consts = {}
     try:
         consts = json.load(open(os.path.join(ROOT, "profiles", "scene_constants_%s.json" % args.workload)))
@@ -429,18 +453,10 @@ def _main(real_stdout):
     ms_opt = sum(s.ms_optimise_phases for s in stats)
     n_launch = sum(int(s.n_patch_launches) for s in stats)
     achieved = (bpp * filled_local / (ms_kernel * 1e-3)) / 1e9 if ms_kernel > 0 and bpp > 0 else None
-    traffic, traffic_src, ncu_context = None, None, None
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "r2_kfrontier_traffic.json")))
-        traffic = tj["dram_bytes_per_launch"]
-        ncu_context = tj.get("ncu_context")
-        traffic_src = tj.get("source")
-    except Exception:
-        pass
     roofline = {"kernel": "k_frontier (persistent cooperative kernel: seeds + every frontier round of the step in one launch; "
                           "one PatchOptimization per thread in large rounds, per warp in small ones)", "bound": "hbm",
                 "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": (achieved / peak) if achieved else None,
-                "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+                "peak_source": peak_src,
                 "algorithmic_bytes_per_filled_px": bpp,
                 "definition": "300 B x N_PSE + 75 B x N_opt + 28 B x N_filled with the oracle's strict-order counts per filled "
                               "pixel (profiles/scene_constants_%s.json) x filled pixels of the launch, / CUDA-event time of the "
@@ -453,15 +469,13 @@ def _main(real_stdout):
                 "grid_barriers_per_launch": sum(int(s.n_grid_barriers) for s in stats) / max(1, n_launch),
                 "impl_sample_sets": sum(int(s.n_sample_sets) for s in stats), "impl_opts": sum(int(s.n_opt) for s in stats),
                 "impl_bytes_300_per_set_GBs": (300.0 * sum(int(s.n_sample_sets) for s in stats) / (ms_kernel * 1e-3) / 1e9) if ms_kernel > 0 else None}
-    if ncu_context:
-        roofline["ncu_context"] = ncu_context      # what actually bounds the kernel, from the committed capture
     # context only: the same launches against the fp32 SIMT peak with SURVEY.md 8(d)'s ~110 kFLOP per reference
     # PatchOptimization (oracle count per filled pixel x filled pixels)
     opf = float(consts.get("opt_per_filled_px", 0.0))
     if ms_kernel > 0 and opf > 0:
         tf = 110e3 * opf * filled_local / (ms_kernel * 1e-3) / 1e12
-        roofline["fp32_context"] = {"achieved_tflops": tf, "peak_tflops": 74.0, "frac": tf / 74.0,
-                                    "note": "148 SM x 128 lanes x 2 x 1.965 GHz (derived, not measured); 110 kFLOP per reference optimisation"}
+        roofline["fp32_context"] = {"achieved_tflops": tf, "peak_tflops": 67.0, "frac": tf / 67.0,
+                                    "note": "H100 SXM data sheet dense FP32 (700 W card; not measured); 110 kFLOP per reference optimisation"}
 
     # ---- cpu_baseline (rank 0): the reference's own CPU dmrecon on this box's host cores, bounded sample ----
     cpu_baseline = None
@@ -508,7 +522,7 @@ def _main(real_stdout):
                            "reference_views_per_gpu": len(refs), "reference_views_total": int(refs_total),
                            "sharding": ("reference views block-sharded over ranks; each rank receives exactly the neighbour images it needs from their owners "
                                         "(NCCL send/recv, %.0f MB per step on rank 0)" % (exchanged["bytes"] / 1e6)) if world > 1 else "single GPU",
-                           "l2": "256 MiB buffer written between steps (L2 flush); the pyramids alone (%.0f MB incl. quad texels) exceed the 126 MB L2" %
+                           "l2": "256 MiB buffer written between steps (L2 flush); the pyramids alone (%.0f MB incl. quad texels) exceed the 50 MB L2" %
                                  (len(needed) * W * H * 20 * 4 / 3 / 1e6),
                            "host_phase": "global view selection + seed lists of step k+1 are computed on a helper thread while the GPU runs step k (b200mvs_plan_views)",
                            "filled_px_per_step": filled_total / args.steps, "swept_px_per_step": int(refs_total) * Ws * Hs,

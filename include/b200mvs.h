@@ -1,5 +1,5 @@
 /*
- * b200mvs - B200-native (sm_100a) dense multi-view-stereo depth-map engine behind the
+ * b200mvs - H100-native (sm_90a) dense multi-view-stereo depth-map engine behind the
  * interface of simonfuhrmann/mve's libs/dmrecon.
  *
  * This is the drop-in boundary: a plain C ABI (no C++/torch types) exported by

@@ -1,4 +1,4 @@
-"""Builds mve_b200/libb200mvs.so (sm_100a) in-tree with nvcc."""
+"""Builds mve_b200/libb200mvs.so (sm_90a) in-tree with nvcc."""
 from __future__ import annotations
 
 import os
@@ -10,7 +10,7 @@ LIB = os.path.join(HERE, "libb200mvs.so")
 SOURCES = [os.path.join(HERE, "csrc", "b200mvs.cu"), os.path.join(HERE, "csrc", "depthmap.cu")]
 DEPS = SOURCES + [os.path.join(HERE, "csrc", "patch_opt.cuh"), os.path.join(HERE, "csrc", "patch_thread.cuh"), os.path.join(HERE, "csrc", "patch_warp.cuh"),
                os.path.join(ROOT, "include", "b200mvs.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v"]
 
 

@@ -1,5 +1,5 @@
 // libb200mvs.so - C ABI of include/b200mvs.h: context, image pyramids, host-side view selection and seeds,
-// frontier (region growing) orchestration and all CUDA kernels.  sm_100a only; no CPU fallback.
+// frontier (region growing) orchestration and all CUDA kernels.  sm_90a only; no CPU fallback.
 #include "../../include/b200mvs.h"
 #include "patch_opt.cuh"
 #include "patch_warp.cuh"
@@ -476,10 +476,10 @@ __global__ void k_export_rgb(const uchar4* __restrict__ src, int w, int h, int p
 // kernels: patch optimisation + frontier
 // ------------------------------------------------------------------------------------------------
 #ifndef OPT_TPB
-#define OPT_TPB 512          // threads per CTA of the patch-optimisation kernels: one CTA per SM shares ONE 64 KB table
+#define OPT_TPB 384          // threads per CTA of the patch-optimisation kernels: one CTA per SM shares ONE 64 KB table
 #endif
 #ifndef OPT_MIN_BLOCKS
-#define OPT_MIN_BLOCKS 1     // CTAs per SM: registers per thread <= 65536 / (OPT_MIN_BLOCKS * OPT_TPB) = 128; shared memory 180 KB per CTA
+#define OPT_MIN_BLOCKS 1     // CTAs per SM: registers per thread <= 65536 / (OPT_MIN_BLOCKS * OPT_TPB) = 170; shared memory 151 KB per CTA
 #endif
 constexpr int OPT_WARPS = OPT_TPB / 32;
 using PatchT = b200mvs::PatchW;    // one warp per patch (latency: small rounds)
@@ -663,7 +663,7 @@ __device__ __forceinline__ unsigned long long ld_relaxed_u64(const unsigned long
 // All CTAs are co-resident (cooperative launch), so a monotone ticket counter is a barrier: the k-th generation is
 // complete when the counter reaches k * gridDim.x.  The wait polls with a RELAXED load: an acquire load in the loop
 // (ld.acquire = LDG + CCTL.IVALL) would invalidate the SM's L1 on every poll and starve the CTAs of the same SM that are
-// still sampling (measured: L1 hit rate 47 % -> profiles/r2_notes.md); one fence after the wait orders the phase.  Data that
+// still sampling; one fence after the wait orders the phase.  Data that
 // other SMs write during the kernel is read with ld.cg everywhere, so no L1 invalidation is needed for correctness.
 __device__ __forceinline__ void grid_barrier(unsigned long long* bar)
 {
@@ -920,7 +920,6 @@ k_frontier(const FrontierParams P)
                 const unsigned k = atomicSub(&P.tile_cnt[bin], 1u) - 1u;
                 P.run2[__ldcg(&P.tile_off[bin]) + k] = e;
             }
-            if (lead) { ctl->sort_cursor = 0ull; ctl->small_cursor = 0ull; }
             PHASE_END(PH_SORT);
             run_cur = P.run2;
         }
@@ -989,7 +988,9 @@ k_frontier(const FrontierParams P)
             }
             P.written[i] = w;
         }
-        if (lead) { ctl->nrun = 0ull; ctl->ticket = 0ull; ctl->ticket2 = 0ull; }
+        // The round's counters are reset here, in a phase in which no thread takes from them: a reset inside the phase that
+        // uses a counter lets CTAs that are still working restart at slot 0 (lost and duplicated entries).
+        if (lead) { ctl->nrun = 0ull; ctl->ticket = 0ull; ctl->ticket2 = 0ull; ctl->sort_cursor = 0ull; ctl->small_cursor = 0ull; }
         if (blockIdx.x == 0) for (int j = threadIdx.x; j < P.n_jobs; j += blockDim.x) P.job_run[j] = 0ull;
         PHASE_END(PH_COMMIT);
         // E: after ALL commits, push the 4-neighbours of every committed pixel (dmrecon.cc:400-431)
@@ -1228,7 +1229,7 @@ unsigned ids_to_slots(const std::vector<int>& gsel, const int32_t* ids, int n, b
 // ------------------------------------------------------------------------------------------------
 extern "C" {
 
-const char* b200mvs_version(void) { return "b200mvs 0.1 (sm_100a)"; }
+const char* b200mvs_version(void) { return "b200mvs 0.1 (sm_90a)"; }
 
 void b200mvs_default_settings(b200mvs_settings* s)
 {

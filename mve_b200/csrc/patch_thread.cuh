@@ -54,7 +54,7 @@ struct PatchT {
     int iter;
     unsigned n_sets;
     // Everything small lives in ONE register (`pk`): the state of a patch stays live across the whole sample loop, and
-    // every register it occupies there is a register the loop spills (profiles/r2_notes.md, "state packing").
+    // every register it occupies there is a register the loop spills.
     //   bits 0-9   flags F_*          bits 10-12 stage        bits 13-15 nsel (size of the selected set)
     //   bits 16-19 p_col_ok           bits 20-23 p_der_ok     (per selected view: colour / derivative samples valid in the last pass)
     //   bits 24-27 |NCC - oldNCC| > minRefineDiff per selected view, taken when the last pass overwrote the NCC (the
@@ -314,7 +314,7 @@ struct PatchT {
                 // The sample loop is software-pipelined: the geometry of sample k+1 is evaluated and its two loads (quad texel
                 // of the neighbour, master texel) are issued BEFORE sample k is processed, so their latency is covered by the
                 // ~150 instructions of table look-ups, interpolation and sums of sample k (an un-pipelined loop stalled on the
-                // first use of each load, profiles/r2_notes.md).
+                // first use of each load).
                 const uchar4* mptr = job->ref_img + (size_t)(y0 - 2) * job->ref_pitch + (x0 - 2);
                 const int mskip = job->ref_pitch - 5;
                 float ndi = -2.f, ndj = -2.f;              // offsets of the NEXT sample

@@ -9,7 +9,15 @@ Outputs (all under tests/golden/):
       patch_in / patch_out     inputs and mvs::PatchOptimization results through oracle/_ref/ref_harness
       depth_v / conf_v / dz_v  maps written by oracle/_ref/dmrecon for views v (apps/dmrecon CLI, unmodified)
       undist_v                 pyramid level `scale` written by the reference (scale != 0 only)
+  C2_view5_ref.npz, C5r_view3_ref.npz   reference CLI maps at BASELINE size, reduced by sampled_map()
+  depthmap_ops_ref.npz    libs/mve/depthmap.cc results for tests/test_gpu_depthmap_ops.py
+  T0s77_ref.npz           mvs::PatchOptimization results on a scene generated with seed 77
+  T0_ply_ref.npz          .xf files and PLY headers written by the reference CLI with -p
+
+`python tests/golden/make_golden.py [tiny] [baseline_size] [depthmap_ops] [fresh_scene_patches] [ply]` mints only the
+named groups (default: all).
 """
+import hashlib
 import os
 import re
 import shutil
@@ -128,10 +136,117 @@ def mint(name, map_views, n_patches=1500):
         shutil.rmtree(tmp, ignore_errors=True)
 
 
+def sha256(a):
+    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
+
+
+def sampled_map(maps, n_sample, seed=0):
+    """A full-size reference map reduced for storage: the fill mask in full (bit-packed) and depth / conf / dz at a seeded
+    sample of the filled pixels."""
+    depth = maps["depth"]
+    filled = np.flatnonzero(depth > 0)
+    idx = np.sort(np.random.default_rng(seed).choice(filled, size=min(n_sample, len(filled)), replace=False)).astype(np.int32)
+    return dict(shape=np.asarray(depth.shape, np.int32), mask=np.packbits(depth.reshape(-1) > 0), idx=idx,
+                depth=depth.reshape(-1)[idx], conf=maps["conf"].reshape(-1)[idx], dz=maps["dz"].reshape(-1, 2)[idx])
+
+
+def mint_baseline_size():
+    """Reference CLI maps of the BASELINE-sized views of tests/test_gpu_parity_baseline_size.py (scenes generated on the CPU)."""
+    from tests.test_gpu_parity_baseline_size import C5R
+    from tests.util import reference_cli_maps
+    for name, s, view in (("C2_view5", synth.make_scene("C2"), 5), ("C5r_view3", synth.make_scene("C5", **C5R), 3)):
+        ref = reference_cli_maps(s, [view])[view]
+        np.savez_compressed(os.path.join(GOLD, "%s_ref.npz" % name), **sampled_map(ref, 4096))
+        print(name, int((ref["depth"] > 0).sum()), "filled px")
+
+
+def mint_depthmap_ops():
+    """libs/mve/depthmap.cc through ref_harness dmops on the cases of tests/test_gpu_depthmap_ops.py: bit-exact results as
+    SHA-256 digests, float results of triangulate at up to 256 seeded vertices."""
+    from tests.test_gpu_depthmap_ops import CLEANUP_THRES, TRI_CASES, depth_case, tri_inputs
+    harness = os.path.join(REF, "ref_harness")
+    data = {}
+    with tempfile.TemporaryDirectory() as tmp:
+        for kind in ("golden", "ragged", "large"):
+            dm, cm = depth_case(kind)
+            h, w = dm.shape
+            dm.tofile(os.path.join(tmp, "dm.f32")); cm.tofile(os.path.join(tmp, "cm.f32"))
+            subprocess.run([harness, "dmops", "confclean", str(w), str(h), os.path.join(tmp, "dm.f32"), os.path.join(tmp, "cm.f32"),
+                            os.path.join(tmp, "cc.f32")], check=True)
+            data["confclean_%s" % kind] = sha256(np.fromfile(os.path.join(tmp, "cc.f32"), np.float32))
+            for thres in CLEANUP_THRES:
+                subprocess.run([harness, "dmops", "cleanup", str(w), str(h), str(thres), os.path.join(tmp, "dm.f32"),
+                                os.path.join(tmp, "cl.f32")], check=True)
+                data["cleanup_%s_%d" % (kind, thres)] = sha256(np.fromfile(os.path.join(tmp, "cl.f32"), np.float32))
+        for kind, dd, color in TRI_CASES:
+            dm, invproj, ci = tri_inputs(kind, color)
+            h, w = dm.shape
+            dm.tofile(os.path.join(tmp, "dm.f32"))
+            cpath = "-"
+            if ci is not None:
+                cpath = os.path.join(tmp, "ci.u8"); ci.tofile(cpath)
+            subprocess.run([harness, "dmops", "triangulate", str(w), str(h), repr(dd), os.path.join(tmp, "dm.f32"), cpath, "3"] +
+                           [repr(float(v)) for v in invproj] + [os.path.join(tmp, "out")], check=True)
+            rd = lambda ext, t: np.fromfile(os.path.join(tmp, "out." + ext), t)      # noqa: E731
+            vids, faces, confs = rd("vids", np.uint32), rd("faces", np.uint32), rd("confs", np.float32)
+            verts, nrm, scl, cols = rd("verts", np.float32).reshape(-1, 3), rd("normals", np.float32).reshape(-1, 3), \
+                rd("scales", np.float32), rd("colors", np.float32)
+            key = "tri_%s_%g_%d" % (kind, dd, int(color))
+            pick = np.sort(np.random.default_rng(0).choice(len(verts), size=min(256, len(verts)), replace=False)).astype(np.int32)
+            data[key + "_n"] = np.asarray([len(verts), len(faces) // 3], np.int64)
+            data[key + "_sha"] = np.asarray([sha256(vids), sha256(faces), sha256(confs)])
+            data[key + "_pick"] = pick
+            data[key + "_verts"], data[key + "_normals"], data[key + "_scales"] = verts[pick], nrm[pick], scl[pick]
+            data[key + "_scales_absmax"] = np.float32(np.abs(scl).max())
+            data[key + "_verts_absmax"] = np.float32(np.abs(verts).max())
+            if cols.size:
+                data[key + "_colors"] = cols.reshape(-1, 4)[pick]
+    np.savez_compressed(os.path.join(GOLD, "depthmap_ops_ref.npz"), **data)
+    print("depthmap ops", len(data), "entries")
+
+
+def mint_fresh_scene_patches():
+    """mvs::PatchOptimization of the reference on a slice of the oracle's trace of a scene that no other fixture uses."""
+    from tests.test_oracle_vs_reference import fresh_scene_trace
+    s, tin = fresh_scene_trace()
+    with tempfile.TemporaryDirectory() as tmp:
+        synth.write_mve_scene(s, tmp)
+        fin, fout = os.path.join(tmp, "in.bin"), os.path.join(tmp, "out.bin")
+        tin.tofile(fin)
+        subprocess.run([os.path.join(REF, "ref_harness"), "patches", tmp, "1", "0", "4", fin, fout], check=True, capture_output=True)
+        out = np.fromfile(fout, dtype=O.PATCH_OUT)
+    np.savez_compressed(os.path.join(GOLD, "T0s77_ref.npz"), patch_in=tin, conf=out["conf"], depth=out["depth"],
+                        local_ids=out["local_ids"].astype(np.int8))
+    print("fresh scene", len(tin), "patches")
+
+
+def mint_ply():
+    """.xf files and PLY header / element counts written by the reference CLI with -p (tests/test_gpu_dropin_cli.py)."""
+    from tests.test_gpu_dropin_cli import PLY_VIEWS, ply_cmd, read_ply_header
+    s = synth.load_scene_npz(os.path.join(GOLD, "T0_scene.npz"))
+    data = {}
+    with tempfile.TemporaryDirectory() as tmp:
+        synth.write_mve_scene(s, tmp)
+        subprocess.run(ply_cmd(os.path.join(REF, "dmrecon"), s, tmp), check=True, capture_output=True,
+                       env=dict(os.environ, OMP_NUM_THREADS="2"))
+        for v in PLY_VIEWS:
+            name = "mvs-%04d-L%d" % (v, s.scale)
+            nv, nf, head = read_ply_header(os.path.join(tmp, "plyout", name + ".ply"))
+            data["ply_%d" % v] = np.asarray([nv, nf], np.int64)
+            data["ply_props_%d" % v] = np.asarray([l for l in head.splitlines() if l.startswith("property")])
+            data["xf_%d" % v] = np.asarray(open(os.path.join(tmp, "plyout", name + ".xf")).read())
+    np.savez_compressed(os.path.join(GOLD, "T0_ply_ref.npz"), **data)
+
+
 if __name__ == "__main__":
-    np.save(os.path.join(GOLD, "srgb2lin.npy"), parse_lut())
-    mint("T0", [0, 3])
-    mint("T1", [4])
-    mint("T2", [0])
-    mint("T4", [1])
-    mint_gvs_only("T3")
+    parts = sys.argv[1:] or ["tiny", "baseline_size", "depthmap_ops", "fresh_scene_patches", "ply"]
+    if "tiny" in parts:
+        np.save(os.path.join(GOLD, "srgb2lin.npy"), parse_lut())
+        mint("T0", [0, 3])
+        mint("T1", [4])
+        mint("T2", [0])
+        mint("T4", [1])
+        mint_gvs_only("T3")
+    for p in parts:
+        if p != "tiny":
+            globals()["mint_" + p]()

@@ -1,7 +1,7 @@
 """The drop-in itself (-m gpu): the reference's UNMODIFIED CLI driver (apps/dmrecon/dmrecon.cc, compiled from the
 reference tree) linked against our mvs::DMRecon shim + libb200mvs.so instead of libmve_dmrecon.a, run on an MVE scene
 directory, must leave the same embeddings on disk as the reference binary did (golden maps minted by
-tests/golden/make_golden.py from oracle/_ref/dmrecon).  Skipped when shim/_build/dmrecon_b200 was not built."""
+tests/golden/make_golden.py from the reference CLI).  Skipped when oracle/_ref/shim/dmrecon_b200 was not built."""
 import os
 import subprocess
 import tempfile
@@ -12,10 +12,10 @@ import pytest
 from tests.util import ROOT, golden_ref, golden_scene, map_stats
 
 pytestmark = pytest.mark.gpu
-CLI = os.path.join(ROOT, "shim", "_build", "dmrecon_b200")
+CLI = os.path.join(ROOT, "oracle", "_ref", "shim", "dmrecon_b200")
 
 
-@pytest.mark.skipif(not os.path.exists(CLI), reason="shim/_build/dmrecon_b200 not built (needs /root/reference at build time)")
+@pytest.mark.skipif(not os.path.exists(CLI), reason="oracle/_ref/shim/dmrecon_b200 not built (needs the reference sources at build time)")
 @pytest.mark.parametrize("name,views", [("T0", [0, 3]), ("T1", [4])])
 def test_cli_writes_reference_layout(name, views):
     from mve_b200 import synth
@@ -46,47 +46,48 @@ def test_cli_writes_reference_layout(name, views):
         assert out2.returncode == 0
 
 
-REF_CLI = os.path.join(ROOT, "oracle", "_ref", "dmrecon")
+PLY_VIEWS = (0, 3)
 
 
-def _read_ply_vertices(path):
-    """Binary little-endian PLY of mve::geom::save_ply_view: returns (n_vertices, n_faces, vertex block bytes)."""
+def ply_cmd(exe, s, scene_dir):
+    return [exe, "-s%d" % s.scale, "--progress=silent", "--force", "-p", "--plydest=plyout",
+            "-l" + ",".join(str(v) for v in PLY_VIEWS), scene_dir]
+
+
+def read_ply_header(path):
+    """Binary little-endian PLY of mve::geom::save_ply_view: returns (n_vertices, n_faces, header text)."""
     raw = open(path, "rb").read()
     end = raw.index(b"end_header\n") + len(b"end_header\n")
     head = raw[:end].decode("ascii", "replace")
     nv = int([l for l in head.splitlines() if l.startswith("element vertex")][0].split()[-1])
     nf = int(([l for l in head.splitlines() if l.startswith("element face")] or ["element face 0"])[0].split()[-1])
-    return nv, nf, head, raw[end:]
+    return nv, nf, head
 
 
-@pytest.mark.skipif(not (os.path.exists(CLI) and os.path.exists(REF_CLI)), reason="drop-in or reference CLI not built")
+@pytest.mark.skipif(not os.path.exists(CLI), reason="oracle/_ref/shim/dmrecon_b200 not built")
 def test_cli_writes_ply_like_the_reference():
     """-p / --writeply (settings.writePlyFile, plyPath; dmrecon.cc:109-117, single_view.cc:123-138): the drop-in writes
     mvs-<id>-L<s>.ply / .xf through the same libmve writers; vertex and face counts follow the depth map, so they agree with
-    the reference's file up to the pixels on which the maps differ, the .xf files are identical."""
+    the reference's file (golden T0_ply_ref.npz) up to the pixels on which the maps differ, the .xf files are identical."""
     from mve_b200 import synth
     s = golden_scene("T0")
-    with tempfile.TemporaryDirectory() as t1, tempfile.TemporaryDirectory() as t2:
-        outs = []
-        for exe, tmp in ((CLI, t1), (REF_CLI, t2)):
-            synth.write_mve_scene(s, tmp)
-            cmd = [exe, "-s%d" % s.scale, "--progress=silent", "--force", "-p", "--plydest=plyout", "-l0,3", tmp]
-            out = subprocess.run(cmd, capture_output=True, text=True, timeout=600, env=dict(os.environ, OMP_NUM_THREADS="2"))
-            assert out.returncode == 0, out.stdout + out.stderr
-            outs.append(out.stdout)
-        for v in (0, 3):
+    ref = golden_ref("T0_ply")
+    with tempfile.TemporaryDirectory() as tmp:
+        synth.write_mve_scene(s, tmp)
+        out = subprocess.run(ply_cmd(CLI, s, tmp), capture_output=True, text=True, timeout=600, env=dict(os.environ, OMP_NUM_THREADS="2"))
+        assert out.returncode == 0, out.stdout + out.stderr
+        for v in PLY_VIEWS:
             name = "mvs-%04d-L%d" % (v, s.scale)
-            a = os.path.join(t1, "plyout", name + ".ply")
-            b = os.path.join(t2, "plyout", name + ".ply")
-            assert os.path.exists(a) and os.path.exists(b)
-            assert open(os.path.join(t1, "plyout", name + ".xf")).read() == open(os.path.join(t2, "plyout", name + ".xf")).read()
-            nva, nfa, ha, _ = _read_ply_vertices(a)
-            nvb, nfb, hb, _ = _read_ply_vertices(b)
-            assert [l for l in ha.splitlines() if l.startswith("property")] == [l for l in hb.splitlines() if l.startswith("property")]
+            a = os.path.join(tmp, "plyout", name + ".ply")
+            assert os.path.exists(a)
+            assert open(os.path.join(tmp, "plyout", name + ".xf")).read() == str(ref["xf_%d" % v])
+            nva, nfa, ha = read_ply_header(a)
+            nvb, nfb = (int(x) for x in ref["ply_%d" % v])
+            assert [l for l in ha.splitlines() if l.startswith("property")] == ref["ply_props_%d" % v].tolist()
             assert abs(nva - nvb) <= 0.01 * nvb + 5 and abs(nfa - nfb) <= 0.03 * nfb + 20, (nva, nvb, nfa, nfb)
 
 
-@pytest.mark.skipif(not os.path.exists(CLI), reason="shim/_build/dmrecon_b200 not built")
+@pytest.mark.skipif(not os.path.exists(CLI), reason="oracle/_ref/shim/dmrecon_b200 not built")
 def test_cli_batches_the_views_in_flight():
     """The OpenMP threads of the unmodified driver (apps/dmrecon/dmrecon.cc:285) are combined into ONE b200mvs_reconstruct per
     GPU: with 6 views on 6 threads every 'Reconstructed view' line reports the features of the whole batch."""

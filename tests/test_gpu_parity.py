@@ -6,7 +6,7 @@ Stated tolerances (fp32 path, DESIGN.md "Parity"):
   * integer results - pyramid bytes, global view selection, per-patch local view ids - are exact; discrete
     per-patch decisions (success / selected views) may flip on <= 0.2 % of patches through thresholded float tests;
   * patch level (same inputs) vs the reference's own results: depth rel err p99 <= 1e-6, p99.9 <= 1e-4, <= 1e-5 on >= 99.7 %;
-    conf abs p99 <= 2e-5; dz abs p99 <= 1e-6 (measured: profiles/r2_patch_parity.json);
+    conf abs p99 <= 2e-5; dz abs p99 <= 1e-6 (tools/patch_parity.py prints the measured figures);
   * map level vs the restatement under the SAME frontier schedule: fill IoU >= 0.995, depth rel p99 <= 2e-3;
   * map level vs the reference CLI (strict priority order): fill IoU >= 0.99, depth rel p50 <= 5e-4, p99 <= 5e-3,
     conf abs p99 <= 2e-2 - the size of the effect of the processing order alone, measured on the CPU in
@@ -79,9 +79,8 @@ def test_patches_vs_reference_golden(ctx, name, mode):
     g.set_patch_mode(0)
     c = patch_compare(got, ref["patch_out"])
     n = c["n"]
-    # measured on B200 (tools/patch_parity.py, profiles/r2_patch_parity.json): 0 discrete mismatches, depth rel p99 1e-7..3e-7,
-    # within 1e-5 on 99.7..100 % of the patches (SURVEY 8c asks 99.9 %: met by the warp implementation on 3 of 4 scenes, by
-    # the thread implementation on 2 of 4; the rest are patches whose Gauss-Newton stopped one iteration apart)
+    # SURVEY 8c asks for 1e-5 on 99.9 % of the patches; the bound below leaves room for the patches whose Gauss-Newton
+    # stopped one iteration apart from the reference's (tools/patch_parity.py prints the measured figures)
     assert c["ok_mismatch"] <= max(1, 0.001 * n), c["ok_mismatch"]
     assert c["ids_mismatch"] <= max(1, 0.001 * n), c["ids_mismatch"]
     assert np.percentile(c["rel"], 99) < 1e-6
@@ -193,6 +192,25 @@ def test_deterministic(ctx):
     for j in range(2):
         for k in ("depth", "conf", "dz", "normal", "view_ids"):
             assert (a[j][k] == b[j][k]).all()
+
+
+def test_deterministic_mixed_rounds(ctx):
+    """Repeated calls give bitwise identical maps when rounds mix both device implementations: with thread_min 256 on all
+    9 views many rounds run some views one thread per patch (tile-grouped) and the others one warp per patch (the list
+    behind them)."""
+    s, g, o = ctx("T1")
+    gs, _ = _settings(s)
+    views = list(range(s.n_views))
+    g.set_patch_mode(0, 256)
+    try:
+        a, _ = g.reconstruct(gs, views)
+        for _ in range(3):
+            b, _ = g.reconstruct(gs, views)
+            for j in range(len(views)):
+                for k in ("depth", "conf", "dz", "normal", "view_ids"):
+                    assert (a[j][k] == b[j][k]).all(), (views[j], k)
+    finally:
+        g.set_patch_mode(0, -1)
 
 
 def test_config_C1_full_size_vs_oracle():

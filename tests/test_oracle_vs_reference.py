@@ -9,14 +9,12 @@ the restatement with strict IEEE evaluation; the reference differs from ITSELF b
 compiler flags (SURVEY.md §6: depth rel p99 3.2e-4, max 3.1e-3 at map level).  Integer results must be equal.
 """
 import os
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
 from oracle import oracle_py as O
-from tests.util import GOLD, ROOT, golden_ref, golden_scene, map_stats, patch_compare
+from tests.util import GOLD, golden_ref, golden_scene, map_stats, patch_compare
 
 
 @pytest.fixture(scope="module")
@@ -106,22 +104,27 @@ def test_maps_vs_reference_cli(osc, name, views):
         assert np.percentile(np.abs(ref["dz_%d" % v] - r["dz"])[both], 99) < tol["dz"]
 
 
-@pytest.mark.skipif(not os.path.exists(os.path.join(ROOT, "oracle", "_ref", "ref_harness")),
-                    reason="oracle/_ref not built (needs /root/reference)")
-def test_live_reference_patches_on_fresh_scene():
-    """Live run of the compiled reference on a scene that is NOT in the fixtures."""
+def fresh_scene_trace():
+    """A scene generated with another seed than the T* fixtures and the inputs of up to 3000 PatchOptimizations of the
+    oracle's strict-order reconstruction of view 1."""
     from mve_b200 import synth
+    s = synth.make_scene("T0", seed=77, features=200)
+    r = O.OracleScene(s).reconstruct(O.default_settings(scale=0, nr_recon_neighbors=4), 1, trace_cap=3000)
+    return s, r["trace_in"]
+
+
+def test_reference_patches_on_fresh_scene():
+    """The reference's PatchOptimization results (ref_harness, golden T0s77_ref.npz) on a scene whose images, cameras and
+    features are not those of the other fixtures, vs the restatement on the same inputs."""
+    from mve_b200 import synth
+    ref = golden_ref("T0s77")
     s = synth.make_scene("T0", seed=77, features=200)
     sc = O.OracleScene(s)
     st = O.default_settings(scale=0, nr_recon_neighbors=4)
-    r = sc.reconstruct(st, 1, trace_cap=3000)
-    with tempfile.TemporaryDirectory() as tmp:
-        synth.write_mve_scene(s, tmp)
-        fin, fout = os.path.join(tmp, "in.bin"), os.path.join(tmp, "out.bin")
-        r["trace_in"].tofile(fin)
-        subprocess.run([os.path.join(ROOT, "oracle", "_ref", "ref_harness"), "patches", tmp, "1", "0", "4", fin, fout],
-                       check=True, capture_output=True)
-        ref_out = np.fromfile(fout, dtype=O.PATCH_OUT)
-    c = patch_compare(r["trace_out"], ref_out)
+    got = sc.optimize_patches(st, 1, sc.global_view_selection(st, 1), ref["patch_in"])
+    want = np.zeros(len(got), O.PATCH_OUT)
+    want["conf"], want["depth"], want["local_ids"] = ref["conf"], ref["depth"], ref["local_ids"]
+    c = patch_compare(got, want)
+    assert c["n"] > 1000
     assert c["ok_mismatch"] <= 3 and c["ids_mismatch"] <= 3
     assert np.percentile(c["rel"], 99) < 2e-5

@@ -63,6 +63,25 @@ def reference_cli_maps(scene, views, threads=None):
     return out
 
 
+def map_parity_sampled(ref, got):
+    """map_parity against a stored reference map (tests/golden/make_golden.py sampled_map): fill figures on the whole
+    mask, depth / conf / dz figures on the stored sample of reference pixels that `got` fills too."""
+    shape = tuple(int(x) for x in ref["shape"])
+    m_ref = np.unpackbits(ref["mask"], count=shape[0] * shape[1]).astype(bool)
+    m_got = got["depth"].reshape(-1) > 0
+    n_ref = int(m_ref.sum())
+    iou = (m_ref & m_got).sum() / max(1, (m_ref | m_got).sum())
+    both = m_got[ref["idx"]]
+    idx = ref["idx"][both]
+    rel = np.abs(ref["depth"][both] - got["depth"].reshape(-1)[idx]) / ref["depth"][both]
+    dz = np.abs(ref["dz"][both] - got["dz"].reshape(-1, 2)[idx]).max(-1)
+    return dict(iou=float(iou), fill_ratio_diff=float(abs(int(m_got.sum()) - n_ref) / max(1, n_ref)),
+                depth_rel_p50=float(np.percentile(rel, 50)), depth_rel_p99=float(np.percentile(rel, 99)),
+                depth_rel_le_1e3=float((rel <= 1e-3).mean()), depth_rel_le_1e2=float((rel <= 1e-2).mean()),
+                conf_abs_p99=float(np.percentile(np.abs(ref["conf"][both] - got["conf"].reshape(-1)[idx]), 99)),
+                dz_abs_p99=float(np.percentile(dz, 99)), n_both=int(both.sum()))
+
+
 def map_parity(ref, got):
     """SURVEY.md 8c map-level figures of `got` against `ref` (dicts with depth, conf, dz)."""
     iou, rel, both = map_stats(ref["depth"], got["depth"])

@@ -21,7 +21,7 @@ def build(cfgs):
         tpb, minb = parts[0], parts[1]
         extra = parts[2:]
         out = os.path.join(VAR, "lib_%s_%s%s.so" % (tpb, minb, "".join("_" + e.replace("-D", "").replace("=", "") for e in extra)))
-        cmd = ["/usr/local/cuda/bin/nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
+        cmd = ["/usr/local/cuda/bin/nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
                "-shared", "-DOPT_TPB=" + tpb, "-DOPT_MIN_BLOCKS=" + minb] + extra + ["-o", out, os.path.join(ROOT, "mve_b200", "csrc", "b200mvs.cu"), os.path.join(ROOT, "mve_b200", "csrc", "depthmap.cu")]
         subprocess.check_call(cmd)
         print(out)

@@ -1,4 +1,4 @@
-"""Summarise an .ncu-rep (raw page) into the few numbers DESIGN.md / profiles/ quote. usage: ncu_summary.py rep [out.md]"""
+"""Summarise an .ncu-rep (raw page) into a few headline numbers. usage: ncu_summary.py rep [out.md]"""
 import csv
 import io
 import subprocess
