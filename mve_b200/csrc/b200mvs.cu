@@ -1231,6 +1231,18 @@ extern "C" {
 
 const char* b200mvs_version(void) { return "b200mvs 0.1 (sm_90a)"; }
 
+#if defined(B200MVS_SWEEP_MIX)
+// Diagnostic build only: copies the sweep-mix histogram of the current device (patch_thread.cuh, g_sweep_mix) to out[0..n).
+int b200mvs_sweep_mix(uint64_t* out, int n)
+{
+    if (!out || n <= 0) return -1;
+    unsigned long long h[128];
+    if (cudaMemcpyFromSymbol(h, b200mvs::g_sweep_mix, sizeof(h)) != cudaSuccess) return -1;
+    for (int i = 0; i < n && i < 128; ++i) out[i] = h[i];
+    return 0;
+}
+#endif
+
 void b200mvs_default_settings(b200mvs_settings* s)
 {
     if (!s) return;
