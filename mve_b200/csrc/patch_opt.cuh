@@ -77,12 +77,24 @@ struct PatchOut { float conf, depth, dzI, dzJ, nx, ny, nz; unsigned slots; int i
 // square root sequences.  The reference itself is built with -funsafe-math-optimizations (Makefile.inc:5), i.e. without
 // IEEE guarantees for these operations; the effect on parity is measured by tests/test_gpu_parity.py.  Everything that
 // decides integers on the host (global view selection, seeds, pyramid) stays IEEE.
+// Pinned roundings: a fused multiply-add, a product and a sum that the compiler neither contracts nor splits.  Where the
+// per-sample code of PatchT is written with them, its values do not depend on how the loop around it is arranged (the
+// compiler contracts a * b + c only when both halves land in the same basic block).  The host emulation does not fuse
+// anywhere (g++ in ISO mode, no FMA), so there they are the plain expressions.
 #if defined(B200MVS_HOST_EMU)
 __device__ __forceinline__ float rcp_fast(float x) { return 1.f / x; }
 __device__ __forceinline__ float rsqrt_fast(float x) { return 1.f / sqrtf(x); }
+__device__ __forceinline__ float fma_rn(float a, float b, float c) { return a * b + c; }
+__device__ __forceinline__ float mul_rn(float a, float b) { return a * b; }
+__device__ __forceinline__ float add_rn(float a, float b) { return a + b; }
+__device__ __forceinline__ float sub_rn(float a, float b) { return a - b; }
 #else
 __device__ __forceinline__ float rcp_fast(float x) { float r; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
 __device__ __forceinline__ float rsqrt_fast(float x) { float r; asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
+__device__ __forceinline__ float fma_rn(float a, float b, float c) { return __fmaf_rn(a, b, c); }
+__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
+__device__ __forceinline__ float sub_rn(float a, float b) { return __fsub_rn(a, b); }
 #endif
 
 // sRGB code value (byte K of `w`) -> linear, through the lane-replicated table in shared memory (mvs_tools.cc:21-95).  Replica r of
