@@ -506,6 +506,14 @@ __device__ __forceinline__ Entry load_entry(const Entry* p)       // lists are r
     return e;
 }
 
+__device__ __forceinline__ PatchIn patch_in(const Entry& e)
+{
+    PatchIn pi;
+    pi.x = e.xy & 0xFFFF; pi.y = (e.xy >> 16) & 0xFFFF;
+    pi.depth = e.depth; pi.dzI = e.dzI; pi.dzJ = e.dzJ; pi.slots = e.slots;
+    return pi;
+}
+
 __device__ __forceinline__ unsigned long long global_timer_ns()
 {
     unsigned long long t;
@@ -525,10 +533,7 @@ __device__ __forceinline__ void optimise_entries(PatchT& p, const Entry* list, P
         w = __shfl_sync(FULL, w, 0);
         if (w >= n) break;
         const Entry e = load_entry(&list[w]);
-        PatchIn pi;
-        pi.x = e.xy & 0xFFFF; pi.y = (e.xy >> 16) & 0xFFFF;
-        pi.depth = e.depth; pi.dzI = e.dzI; pi.dzJ = e.dzJ; pi.slots = e.slots;
-        p.begin(&jobs[e.jobdir & 0xFFFFFF], pi);
+        p.begin(&jobs[e.jobdir & 0xFFFFFF], patch_in(e));
         ++opts;
         while (!p.step()) {}
         PatchOut po;
@@ -565,10 +570,7 @@ __device__ __forceinline__ void optimise_entries_t(PatchT1& p, const Entry* list
             if (w >= n) break;
             idx = w;
             const Entry e = load_entry(&list[w]);
-            PatchIn pi;
-            pi.x = e.xy & 0xFFFF; pi.y = (e.xy >> 16) & 0xFFFF;
-            pi.depth = e.depth; pi.dzI = e.dzI; pi.dzJ = e.dzJ; pi.slots = e.slots;
-            p.begin(&jobs[e.jobdir & 0xFFFFFF], pi);
+            p.begin(&jobs[e.jobdir & 0xFFFFFF], patch_in(e));
             have = true;
             ++opts;
         }
@@ -1230,18 +1232,6 @@ unsigned ids_to_slots(const std::vector<int>& gsel, const int32_t* ids, int n, b
 extern "C" {
 
 const char* b200mvs_version(void) { return "b200mvs 0.1 (sm_90a)"; }
-
-#if defined(B200MVS_SWEEP_MIX)
-// Diagnostic build only: copies the sweep-mix histogram of the current device (patch_thread.cuh, g_sweep_mix) to out[0..n).
-int b200mvs_sweep_mix(uint64_t* out, int n)
-{
-    if (!out || n <= 0) return -1;
-    unsigned long long h[128];
-    if (cudaMemcpyFromSymbol(h, b200mvs::g_sweep_mix, sizeof(h)) != cudaSuccess) return -1;
-    for (int i = 0; i < n && i < 128; ++i) out[i] = h[i];
-    return 0;
-}
-#endif
 
 void b200mvs_default_settings(b200mvs_settings* s)
 {

@@ -1,9 +1,10 @@
-"""The product's DEVICE code on the CPU.  mve_b200/csrc/patch_opt.cuh (the warp-per-patch optimisation kernel body) is
-compiled by g++ against a small SIMT emulation (tests/emu/simt_emu.h: 32 host threads per warp, collectives through a
-barrier) and run on the oracle's execution trace.  This checks the kernel's LOGIC - pass state machine, lane-distributed
-arrays, batched reductions, local view selection and view replacement - without a GPU; last-bit numerics differ from the
-GPU (exact reciprocals, libm).  Inputs (pyramid bytes, calibrations) come from the oracle, which is bit-exact with the
-product's pyramid kernels (tests/test_gpu_parity.py::test_pyramid_bit_exact)."""
+"""The product's DEVICE code on the CPU.  The two patch-optimisation implementations - mve_b200/csrc/patch_warp.cuh (one
+warp per patch, mode 1) and patch_thread.cuh (one thread per patch, mode 2), with the state machine they share in
+patch_opt.cuh - are compiled by g++ against a small SIMT emulation (tests/emu/simt_emu.h: 32 host threads per warp,
+collectives through a barrier) and run on the oracle's execution trace.  This checks the kernels' LOGIC - pass state
+machine, lane-distributed arrays, batched reductions, local view selection and view replacement - without a GPU;
+last-bit numerics differ from the GPU (exact reciprocals, libm).  Inputs (pyramid bytes, calibrations) come from the
+oracle, which is bit-exact with the product's pyramid kernels (tests/test_gpu_parity.py::test_pyramid_bit_exact)."""
 import ctypes as C
 
 import numpy as np

@@ -70,7 +70,7 @@ def test_global_view_selection_exact(ctx, name):
 @pytest.mark.parametrize("name", ["T0", "T1", "T2", "T4"])
 def test_patches_vs_reference_golden(ctx, name, mode):
     """mvs::PatchOptimization results of the compiled reference (ref_harness) on identical inputs, through both device
-    implementations (1: eight lanes per patch, 2: one thread per patch)."""
+    implementations (1: one warp per patch, 2: one thread per patch)."""
     s, g, o = ctx(name)
     ref = golden_ref(name)
     gs, _ = _settings(s)
@@ -116,7 +116,7 @@ def test_patches_vs_oracle_trace(ctx, name, view, mode):
 @pytest.mark.parametrize("thread_min", [0, 1 << 40])
 def test_maps_vs_oracle_same_schedule(ctx, name, view, tol, thread_min):
     """DMRecon::start on the GPU vs the restatement running the identical frontier schedule; every round through the
-    one-thread-per-patch implementation (thread_min 0) or through the eight-lanes-per-patch one (huge thread_min)."""
+    one-thread-per-patch implementation (thread_min 0) or through the one-warp-per-patch one (huge thread_min)."""
     s, g, o = ctx(name)
     gs, os_ = _settings(s)
     g.set_patch_mode(0, thread_min)

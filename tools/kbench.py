@@ -2,7 +2,6 @@
 
     python tools/kbench.py [--steps 3] lib_a.so lib_b.so ...     # each in its own process through B200MVS_LIB
     python tools/kbench.py --build "256 2" "192 2" ...            # cross-compile variants into build_variants/ (here, no GPU)
-    python tools/kbench.py --build "384 1 -DB200MVS_SWEEP_MIX"     # diagnostic: distinct sweep kinds per warp (slow, not a timing)
 """
 import json
 import os
@@ -46,14 +45,6 @@ def run_one(steps, workload, nviews=16):
         thr.append(stt.ms_optimise_thread_phases); srt.append(stt.ms_sort_phases)
     out = dict(lib=os.environ.get("B200MVS_LIB", "default"), ms=min(ms), ms_all=ms, optimise_ms=min(opt), optimise_thread_ms=min(thr), sort_ms=min(srt), filled=filled,
                rounds=int(stt.n_rounds), n_opt=int(stt.n_opt), sets=int(stt.n_sample_sets))
-    L = dmrecon.lib()
-    if hasattr(L, "b200mvs_sweep_mix"):       # -DB200MVS_SWEEP_MIX build: distinct sweep kinds per warp-level sweep
-        import ctypes
-        h = (ctypes.c_uint64 * 128)()
-        if L.b200mvs_sweep_mix(h, 128) == 0 and h[32]:
-            out["sweep_mix"] = dict(warp_sweeps=int(h[32]), lanes_per_sweep=h[33] / h[32],
-                                    distinct_kinds={k: int(h[k]) for k in range(1, 32) if h[k]},
-                                    lane_sweeps_by_kind={k - 64: int(h[k]) for k in range(64, 128) if h[k]})
     print(json.dumps(out), flush=True)
 
 
