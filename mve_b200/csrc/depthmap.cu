@@ -4,7 +4,8 @@
 //     apps/scene2pset (scene2pset.cc:264-328): vertex ids, vertices, colours and faces in EXACTLY the reference's order.
 // All of these are streaming kernels over one depth map; the results are bit-exact for the integer parts (masks, component
 // sizes, vertex ids, faces) and for the float parts that are pure per-pixel functions evaluated in the reference's operation
-// order with IEEE operations (no FMA contraction: __fmul_rn / __fadd_rn).
+// order with IEEE operations (__fmul_rn / __fadd_rn; __fmaf_rn only where the reference build itself contracts and the
+// result decides a face: pixel_footprint).
 #include "../../include/b200mvs.h"
 
 #include <cub/device/device_scan.cuh>
@@ -107,26 +108,36 @@ __device__ __forceinline__ float vec_norm(float x, float y, float z)
 {
     return __fsqrt_rn(__fadd_rn(__fadd_rn(__fadd_rn(0.f, __fmul_rn(x, x)), __fmul_rn(y, y)), __fmul_rn(z, z)));
 }
+// The footprint decides which faces exist, so it repeats the reference build's own arithmetic to the bit: with its flags
+// (-O3 -funsafe-math-optimizations on an FMA target) g++ contracts the ray and the squared norm of pixel_footprint into
+// rx = fma(m0, vx, fma(m1, vy, m2)), ry = fma(m3, vx, fma(m4, vy, m5)), rz = fma(m7, vy, fma(m6, vx, m8)) and
+// |r|^2 = fma(rz, rz, rx*rx + ry*ry), then divides (m0 * depth) by the square root.
 __device__ __forceinline__ float pixel_footprint(const InvProj& P, int x, int y, float depth)
 {
-    float rx, ry, rz;
-    pixel_ray(P, x, y, rx, ry, rz);
-    return __fdiv_rn(__fmul_rn(P.m[0], depth), vec_norm(rx, ry, rz));
+    const float vx = (float)x + 0.5f, vy = (float)y + 0.5f;
+    const float rx = __fmaf_rn(P.m[0], vx, __fmaf_rn(P.m[1], vy, P.m[2]));
+    const float ry = __fmaf_rn(P.m[3], vx, __fmaf_rn(P.m[4], vy, P.m[5]));
+    const float rz = __fmaf_rn(P.m[7], vy, __fmaf_rn(P.m[6], vx, P.m[8]));
+    const float sq = __fmaf_rn(rz, rz, __fadd_rn(__fmul_rn(rx, rx), __fmul_rn(ry, ry)));
+    return __fdiv_rn(__fmul_rn(P.m[0], depth), __fsqrt_rn(sq));
 }
 
 // corner j of the 2x2 block at i: pixel i + (j % 2) + width * (j / 2); the four candidate triangles (depthmap.cc:247-250)
 __constant__ int c_tris[4][3] = {{0, 2, 1}, {0, 3, 1}, {0, 2, 3}, {1, 2, 3}};
 
-__device__ __forceinline__ bool is_depthdisc(const float* widths, const float* depths, float dd_factor, int i1, int i2)
+// dd_diag is the diagonal factor `dd_factor *= MATH_SQRT2` of depthmap.cc:198: a float times a double literal, so the
+// reference rounds the product through double.  The host computes it once (b200mvs_depthmap_pointset).
+__device__ __forceinline__ bool is_depthdisc(const float* widths, const float* depths, float dd_factor, float dd_diag, int i1, int i2)
 {
     int i_min = i1, i_max = i2;
     if (depths[i2] < depths[i1]) { i_min = i2; i_max = i1; }
-    if (i1 + i2 == 3) dd_factor = __fmul_rn(dd_factor, 1.41421356237309504880f);      // MATH_SQRT2 (diagonal)
-    return __fadd_rn(depths[i_max], -depths[i_min]) > __fmul_rn(widths[i_min], dd_factor);
+    const float dd = i1 + i2 == 3 ? dd_diag : dd_factor;
+    return __fadd_rn(depths[i_max], -depths[i_min]) > __fmul_rn(widths[i_min], dd);
 }
 
 // Which triangles the block at (x, y) issues (depthmap.cc:229-301): low nibble first triangle (1..4, 0 none), high nibble second.
-__device__ __forceinline__ unsigned block_code(const float* __restrict__ dm, int w, int h, int x, int y, const InvProj& P, float dd_factor)
+__device__ __forceinline__ unsigned block_code(const float* __restrict__ dm, int w, int h, int x, int y, const InvProj& P, float dd_factor,
+                                               float dd_diag)
 {
     if (x < 0 || y < 0 || x >= w - 1 || y >= h - 1) return 0u;
     const size_t i = (size_t)y * w + x;
@@ -152,9 +163,9 @@ __device__ __forceinline__ unsigned block_code(const float* __restrict__ dm, int
         for (int j = 0; j < 4; ++j) if (depths[j] != 0.0f) widths[j] = pixel_footprint(P, x + (j % 2), y + (j / 2), depths[j]);
         for (int j = 0; j < 2 && tri[j] != 0; ++j) {
             const int* tv = c_tris[tri[j] - 1];
-            if (is_depthdisc(widths, depths, dd_factor, tv[0], tv[1])) tri[j] = 0;
-            if (is_depthdisc(widths, depths, dd_factor, tv[1], tv[2])) tri[j] = 0;
-            if (is_depthdisc(widths, depths, dd_factor, tv[2], tv[0])) tri[j] = 0;
+            if (is_depthdisc(widths, depths, dd_factor, dd_diag, tv[0], tv[1])) tri[j] = 0;
+            if (is_depthdisc(widths, depths, dd_factor, dd_diag, tv[1], tv[2])) tri[j] = 0;
+            if (is_depthdisc(widths, depths, dd_factor, dd_diag, tv[2], tv[0])) tri[j] = 0;
         }
     }
     return (unsigned)tri[0] | ((unsigned)tri[1] << 4);
@@ -170,12 +181,13 @@ __device__ __forceinline__ bool code_uses(unsigned code, int corner)
     return false;
 }
 
-__global__ void k_tri_codes(const float* __restrict__ dm, int w, int h, InvProj P, float dd_factor, unsigned char* __restrict__ codes)
+__global__ void k_tri_codes(const float* __restrict__ dm, int w, int h, InvProj P, float dd_factor, float dd_diag,
+                            unsigned char* __restrict__ codes)
 {
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y * blockDim.y + threadIdx.y;
     if (x >= w || y >= h) return;
-    codes[(size_t)y * w + x] = (unsigned char)block_code(dm, w, h, x, y, P, dd_factor);
+    codes[(size_t)y * w + x] = (unsigned char)block_code(dm, w, h, x, y, P, dd_factor, dd_diag);
 }
 
 // The reference numbers a vertex when a triangle references its pixel for the first time, blocks in raster order
@@ -287,6 +299,7 @@ __global__ void k_tri_faces(const unsigned char* __restrict__ codes, int w, int 
 // blocks around its pixel; visiting those blocks in raster order (and a block's triangles in emission order) enumerates the
 // faces in ascending face id - the order in which the reference accumulates (mesh.cc:45-119, mesh_info.cc:28-33).
 struct AdjFace { unsigned a, b, c, first, second; };
+constexpr unsigned RING_NONE = 0xFFFFFFFFu;          // confidence ring of a vertex no border ring has reached (yet)
 
 __device__ __forceinline__ int adjacent_faces(const unsigned char* __restrict__ codes, const unsigned* __restrict__ vids, int w, int h,
                                               int px, int py, unsigned v, AdjFace* out)
@@ -361,14 +374,14 @@ __device__ __forceinline__ int classify_vertex(const AdjFace* faces, int n, unsi
 
 __global__ void k_vertex_attributes(const unsigned char* __restrict__ codes, const unsigned* __restrict__ vids, int w, int h,
                                     const float* __restrict__ verts, float scale_factor,
-                                    float* __restrict__ normals, float* __restrict__ scales, unsigned char* __restrict__ ring)
+                                    float* __restrict__ normals, float* __restrict__ scales, unsigned* __restrict__ ring)
 {
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y * blockDim.y + threadIdx.y;
     if (x >= w || y >= h) return;
     const size_t pi = (size_t)y * w + x;
     const unsigned v = vids[pi];
-    if (ring) ring[pi] = 255;
+    if (ring) ring[pi] = RING_NONE;
     if (v == 0xFFFFFFFFu) return;
     AdjFace faces[8];
     const int n = adjacent_faces(codes, vids, w, h, x, y, v, faces);
@@ -418,16 +431,19 @@ __global__ void k_vertex_attributes(const unsigned char* __restrict__ codes, con
 }
 
 // depthmap_mesh_confidences (depthmap.cc:497-548): ring d = vertices at d face-edge hops from a border vertex get d / iterations.
+// One launch per ring.  A ring distance is below the number of vertices (< 2^32), so RING_NONE never collides with one.  A
+// round that reaches a vertex stores its d in *last_hit; once a round reaches none, no later round can, and the host stops.
 __global__ void k_conf_ring(const unsigned char* __restrict__ codes, const unsigned* __restrict__ vids, int w, int h,
-                            const unsigned char* __restrict__ ring_in, unsigned char* __restrict__ ring_out, int d)
+                            const unsigned* __restrict__ ring_in, unsigned* __restrict__ ring_out, unsigned d,
+                            unsigned* __restrict__ last_hit)
 {
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y * blockDim.y + threadIdx.y;
     if (x >= w || y >= h) return;
     const size_t pi = (size_t)y * w + x;
-    unsigned char r = ring_in[pi];
+    unsigned r = ring_in[pi];
     const unsigned v = vids[pi];
-    if (v != 0xFFFFFFFFu && r == 255) {
+    if (v != 0xFFFFFFFFu && r == RING_NONE) {
         AdjFace faces[8];
         const int n = adjacent_faces(codes, vids, w, h, x, y, v, faces);
         // the adjacent vertices are pixels of the 3x3 neighbourhood: look their rings up through their vertex ids
@@ -437,22 +453,23 @@ __global__ void k_conf_ring(const unsigned char* __restrict__ codes, const unsig
                 const int qx = x + dx, qy = y + dy;
                 if ((dx == 0 && dy == 0) || qx < 0 || qy < 0 || qx >= w || qy >= h) continue;
                 const size_t qi = (size_t)qy * w + qx;
-                if (ring_in[qi] != d - 1) continue;
+                if (ring_in[qi] != d - 1u) continue;
                 const unsigned u = vids[qi];
                 for (int i = 0; i < n; ++i) if (faces[i].first == u || faces[i].second == u) { hit = true; break; }
             }
-        if (hit) r = (unsigned char)d;
+        if (hit) { r = d; *last_hit = d; }
     }
     ring_out[pi] = r;
 }
-__global__ void k_conf_write(const unsigned* __restrict__ vids, const unsigned char* __restrict__ ring, size_t n, int iterations, float* __restrict__ confs)
+__global__ void k_conf_write(const unsigned* __restrict__ vids, const unsigned* __restrict__ ring, size_t n, int iterations, float* __restrict__ confs)
 {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const unsigned v = vids[i];
     if (v == 0xFFFFFFFFu) return;
-    const int r = ring[i];
-    confs[v] = r < iterations ? (float)r / (float)iterations : 1.0f;
+    const unsigned r = ring[i];
+    // current * (1 / iterations): the reference build hoists the division of depthmap.cc:527 out of its loop
+    confs[v] = r < (unsigned)iterations ? __fmul_rn((float)r, __frcp_rn((float)iterations)) : 1.0f;
 }
 
 __global__ void k_fill_u32(unsigned* p, unsigned v, size_t n)
@@ -530,7 +547,8 @@ int b200mvs_depthmap_pointset(int device, const float* depth, int w, int h, cons
                               double* device_ms)
 {
     float *d_dm = nullptr, *d_verts = nullptr, *d_colors = nullptr, *d_ctw = nullptr, *d_normals = nullptr, *d_confs = nullptr, *d_scales = nullptr;
-    unsigned char *d_codes = nullptr, *d_color = nullptr, *d_ring0 = nullptr, *d_ring1 = nullptr;
+    unsigned char *d_codes = nullptr, *d_color = nullptr;
+    unsigned *d_ring0 = nullptr, *d_ring1 = nullptr, *d_last_hit = nullptr;
     unsigned long long *d_counts = nullptr, *d_offsets = nullptr;
     unsigned *d_vids = nullptr, *d_faces = nullptr;
     void* d_tmp = nullptr;
@@ -538,7 +556,7 @@ int b200mvs_depthmap_pointset(int device, const float* depth, int w, int h, cons
     auto cleanup = [&]() {
         for (void* p : {(void*)d_dm, (void*)d_verts, (void*)d_colors, (void*)d_ctw, (void*)d_codes, (void*)d_color, (void*)d_counts,
                         (void*)d_offsets, (void*)d_vids, (void*)d_faces, d_tmp, (void*)d_normals, (void*)d_confs, (void*)d_scales,
-                        (void*)d_ring0, (void*)d_ring1}) if (p) cudaFree(p);
+                        (void*)d_ring0, (void*)d_ring1, (void*)d_last_hit}) if (p) cudaFree(p);
         if (e0) cudaEventDestroy(e0);
         if (e1) cudaEventDestroy(e1);
     };
@@ -571,10 +589,14 @@ int b200mvs_depthmap_pointset(int device, const float* depth, int w, int h, cons
     const bool want_conf = confidences && conf_iterations > 0;
     if (normals) DCK(cudaMalloc(&d_normals, max_v * 12));
     if (scales) DCK(cudaMalloc(&d_scales, max_v * 4));
-    if (want_conf) { DCK(cudaMalloc(&d_confs, max_v * 4)); DCK(cudaMalloc(&d_ring0, n)); DCK(cudaMalloc(&d_ring1, n)); }
+    if (want_conf) {
+        DCK(cudaMalloc(&d_confs, max_v * 4)); DCK(cudaMalloc(&d_ring0, n * 4)); DCK(cudaMalloc(&d_ring1, n * 4));
+        DCK(cudaMalloc(&d_last_hit, 4));
+    }
     const dim3 blk(32, 8), grd((w + 31) / 32, (h + 7) / 8);
     DCK(cudaEventRecord(e0));
-    k_tri_codes<<<grd, blk>>>(d_dm, w, h, P, dd_factor, d_codes);
+    const float dd_diag = (float)((double)dd_factor * 1.41421356237309504880);       // MATH_SQRT2, rounded like depthmap.cc:198
+    k_tri_codes<<<grd, blk>>>(d_dm, w, h, P, dd_factor, dd_diag, d_codes);
     DCK(cudaMemsetAsync(d_counts + n, 0, 8));
     k_tri_counts<<<grd, blk>>>(d_codes, w, h, d_counts);
     DCK(cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, d_counts, d_offsets, (int)(n + 1)));
@@ -589,10 +611,19 @@ int b200mvs_depthmap_pointset(int device, const float* depth, int w, int h, cons
     if (normals || scales || want_conf)
         k_vertex_attributes<<<grd, blk>>>(d_codes, d_vids, w, h, d_verts, scale_factor, d_normals, d_scales, d_ring0);
     if (want_conf) {
-        unsigned char *cur = d_ring0, *nxt = d_ring1;
-        for (int d = 1; d < conf_iterations && d < 255; ++d) {
-            k_conf_ring<<<grd, blk>>>(d_codes, d_vids, w, h, cur, nxt, d);
-            unsigned char* t = cur; cur = nxt; nxt = t;
+        // rings 1 .. conf_iterations - 1; every RING_CHECK rounds the host asks whether the last round still reached a
+        // vertex, so a large conf_iterations costs as many launches as the mesh has rings, not conf_iterations
+        constexpr int RING_CHECK = 16;
+        unsigned *cur = d_ring0, *nxt = d_ring1;
+        DCK(cudaMemsetAsync(d_last_hit, 0, 4));
+        for (int d = 1; d < conf_iterations; ++d) {
+            k_conf_ring<<<grd, blk>>>(d_codes, d_vids, w, h, cur, nxt, (unsigned)d, d_last_hit);
+            unsigned* t = cur; cur = nxt; nxt = t;
+            if (d % RING_CHECK == 0) {
+                unsigned last = 0;
+                DCK(cudaMemcpy(&last, d_last_hit, 4, cudaMemcpyDeviceToHost));
+                if (last != (unsigned)d) break;
+            }
         }
         k_conf_write<<<(unsigned)((n + 255) / 256), 256>>>(d_vids, cur, n, conf_iterations, d_confs);
     }

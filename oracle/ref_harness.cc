@@ -217,9 +217,10 @@ static int run_timed(int argc, char** argv)
 /* Depth-map consumers of the reference (libs/mve/depthmap.cc) on raw little-endian buffers:
  *   ref_harness dmops cleanup W H THRES in.f32 out.f32
  *   ref_harness dmops confclean W H in.f32 conf.f32 out.f32
- *   ref_harness dmops triangulate W H DD in.f32 COLOR.u8|- CCH  i0 .. i8  OUTPREFIX
+ *   ref_harness dmops triangulate W H DD in.f32 COLOR.u8|- CCH  i0 .. i8  OUTPREFIX [CONF_ITER [SCALE_FACTOR]]
  *       -> OUTPREFIX.vids (uint32 W*H), .verts (float32 V*3, camera coordinates), .faces (uint32 F*3), .colors (float32 V*4),
- *          .normals (V*3), .confs (V, depthmap_mesh_confidences(mesh, 4)), .scales (V, scene2pset's scale values x 2.5) */
+ *          .normals (V*3), .confs (V, depthmap_mesh_confidences(mesh, CONF_ITER), default 4; empty for 0),
+ *          .scales (V, scene2pset's scale values x SCALE_FACTOR, default 2.5) */
 static std::vector<char> read_all(const char* path)
 {
     std::ifstream in(path, std::ios::binary);
@@ -271,6 +272,8 @@ static int run_dmops(int argc, char** argv)
         mve::TriangleMesh::Ptr mesh = ci != nullptr ? mve::geom::depthmap_triangulate(dm, ci, invproj, dd, &vids)
                                                     : mve::geom::depthmap_triangulate(dm, invproj, dd, &vids);
         const std::string prefix = argv[18];
+        const int conf_iter = argc > 19 ? std::atoi(argv[19]) : 4;
+        const float scale_factor = argc > 20 ? (float)std::atof(argv[20]) : 2.5f;
         write_all(prefix + ".vids", vids.get_data_pointer(), (std::size_t)W * H * 4);
         write_all(prefix + ".verts", mesh->get_vertices().data(), mesh->get_vertices().size() * 12);
         write_all(prefix + ".faces", mesh->get_faces().data(), mesh->get_faces().size() * 4);
@@ -278,7 +281,7 @@ static int run_dmops(int argc, char** argv)
         /* the rest of the per-view work of apps/scene2pset (scene2pset.cc:316-358): normals, boundary confidences, scale */
         mesh->ensure_normals();
         write_all(prefix + ".normals", mesh->get_vertex_normals().data(), mesh->get_vertex_normals().size() * 12);
-        mve::geom::depthmap_mesh_confidences(mesh, 4);
+        mve::geom::depthmap_mesh_confidences(mesh, conf_iter);
         write_all(prefix + ".confs", mesh->get_vertex_confidences().data(), mesh->get_vertex_confidences().size() * 4);
         {
             mve::TriangleMesh::VertexList const& mverts(mesh->get_vertices());
@@ -289,7 +292,7 @@ static int run_dmops(int argc, char** argv)
                 for (std::size_t k = 0; k < vinf.verts.size(); ++k)
                     mvscale[j] += (mverts[j] - mverts[vinf.verts[k]]).norm();
                 mvscale[j] /= static_cast<float>(vinf.verts.size());
-                mvscale[j] *= 2.5f;
+                mvscale[j] *= scale_factor;
             }
             write_all(prefix + ".scales", mvscale.data(), mvscale.size() * 4);
         }

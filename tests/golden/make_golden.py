@@ -11,11 +11,12 @@ Outputs (all under tests/golden/):
       undist_v                 pyramid level `scale` written by the reference (scale != 0 only)
   C2_view5_ref.npz, C5r_view3_ref.npz   reference CLI maps at BASELINE size, reduced by sampled_map()
   depthmap_ops_ref.npz    libs/mve/depthmap.cc results for tests/test_gpu_depthmap_ops.py
+  depthmap_edges_ref.npz  the same at the decision boundaries and edge shapes of tests/test_gpu_depthmap_edges.py
   T0s77_ref.npz           mvs::PatchOptimization results on a scene generated with seed 77
   T0_ply_ref.npz          .xf files and PLY headers written by the reference CLI with -p
 
-`python tests/golden/make_golden.py [tiny] [baseline_size] [depthmap_ops] [fresh_scene_patches] [ply]` mints only the
-named groups (default: all).
+`python tests/golden/make_golden.py [tiny] [baseline_size] [depthmap_ops] [depthmap_edges] [fresh_scene_patches] [ply]`
+mints only the named groups (default: all).
 """
 import hashlib
 import os
@@ -185,8 +186,8 @@ def mint_depthmap_ops():
             cpath = "-"
             if ci is not None:
                 cpath = os.path.join(tmp, "ci.u8"); ci.tofile(cpath)
-            subprocess.run([harness, "dmops", "triangulate", str(w), str(h), repr(dd), os.path.join(tmp, "dm.f32"), cpath, "3"] +
-                           [repr(float(v)) for v in invproj] + [os.path.join(tmp, "out")], check=True)
+            subprocess.run([harness, "dmops", "triangulate", str(w), str(h), repr(dd), os.path.join(tmp, "dm.f32"), cpath,
+                            str(channels(ci))] + [repr(float(v)) for v in invproj] + [os.path.join(tmp, "out")], check=True)
             rd = lambda ext, t: np.fromfile(os.path.join(tmp, "out." + ext), t)      # noqa: E731
             vids, faces, confs = rd("vids", np.uint32), rd("faces", np.uint32), rd("confs", np.float32)
             verts, nrm, scl, cols = rd("verts", np.float32).reshape(-1, 3), rd("normals", np.float32).reshape(-1, 3), \
@@ -203,6 +204,59 @@ def mint_depthmap_ops():
                 data[key + "_colors"] = cols.reshape(-1, 4)[pick]
     np.savez_compressed(os.path.join(GOLD, "depthmap_ops_ref.npz"), **data)
     print("depthmap ops", len(data), "entries")
+
+
+def channels(ci):
+    return 0 if ci is None else (1 if ci.ndim == 2 else ci.shape[2])
+
+
+def mint_depthmap_edges():
+    """libs/mve/depthmap.cc through ref_harness dmops on the cases of tests/test_gpu_depthmap_edges.py, stored like
+    depthmap_ops_ref.npz: SHA-256 digests of the exact results (per cleanup threshold, per confidence iteration count) and
+    the float results at up to 256 seeded vertices."""
+    from tests.test_gpu_depthmap_edges import cleanup_cases, tri_cases
+    harness = os.path.join(REF, "ref_harness")
+    data = {}
+    with tempfile.TemporaryDirectory() as tmp:
+        f = lambda name: os.path.join(tmp, name)      # noqa: E731
+        for name, (dm, cm, thres) in cleanup_cases().items():
+            h, w = dm.shape
+            dm.tofile(f("dm.f32")); cm.tofile(f("cm.f32"))
+            subprocess.run([harness, "dmops", "confclean", str(w), str(h), f("dm.f32"), f("cm.f32"), f("cc.f32")], check=True)
+            data["confclean_%s" % name] = sha256(np.fromfile(f("cc.f32"), np.float32))
+            data["cleanup_%s_thres" % name] = np.asarray(thres, np.int64)
+            for t in thres:
+                subprocess.run([harness, "dmops", "cleanup", str(w), str(h), str(t), f("dm.f32"), f("cl.f32")], check=True)
+                data["cleanup_%s_%d" % (name, t)] = sha256(np.fromfile(f("cl.f32"), np.float32))
+        for name, c in tri_cases().items():
+            dm, ci = c["dm"], c["color"]
+            h, w = dm.shape
+            dm.tofile(f("dm.f32"))
+            cpath = "-"
+            if ci is not None:
+                cpath = f("ci.u8"); ci.tofile(cpath)
+            key = "tri_%s" % name
+            for k, it in enumerate(c["ref_iters"]):
+                subprocess.run([harness, "dmops", "triangulate", str(w), str(h), repr(c["dd"]), f("dm.f32"), cpath, str(channels(ci))]
+                               + [repr(float(v)) for v in c["invproj"]] + [f("out"), str(it), repr(c["scale"])], check=True)
+                rd = lambda ext, t: np.fromfile(f("out." + ext), t)      # noqa: E731
+                data["%s_confs_%d" % (key, it)] = sha256(rd("confs", np.float32))
+                if k:
+                    continue
+                vids, faces = rd("vids", np.uint32), rd("faces", np.uint32)
+                verts, nrm, scl, cols = rd("verts", np.float32).reshape(-1, 3), rd("normals", np.float32).reshape(-1, 3), \
+                    rd("scales", np.float32), rd("colors", np.float32)
+                pick = np.sort(np.random.default_rng(0).choice(len(verts), size=min(256, len(verts)), replace=False)).astype(np.int32)
+                data[key + "_n"] = np.asarray([len(verts), len(faces) // 3], np.int64)
+                data[key + "_sha"] = np.asarray([sha256(vids), sha256(faces)])
+                data[key + "_pick"] = pick
+                data[key + "_verts"], data[key + "_normals"], data[key + "_scales"] = verts[pick], nrm[pick], scl[pick]
+                data[key + "_scales_absmax"] = np.float32(np.abs(scl).max(initial=0))
+                data[key + "_verts_absmax"] = np.float32(np.abs(verts).max(initial=0))
+                if cols.size:
+                    data[key + "_colors"] = cols.reshape(-1, 4)[pick]
+    np.savez_compressed(os.path.join(GOLD, "depthmap_edges_ref.npz"), **data)
+    print("depthmap edges", len(data), "entries")
 
 
 def mint_fresh_scene_patches():
@@ -239,7 +293,7 @@ def mint_ply():
 
 
 if __name__ == "__main__":
-    parts = sys.argv[1:] or ["tiny", "baseline_size", "depthmap_ops", "fresh_scene_patches", "ply"]
+    parts = sys.argv[1:] or ["tiny", "baseline_size", "depthmap_ops", "depthmap_edges", "fresh_scene_patches", "ply"]
     if "tiny" in parts:
         np.save(os.path.join(GOLD, "srgb2lin.npy"), parse_lut())
         mint("T0", [0, 3])
