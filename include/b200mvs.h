@@ -30,6 +30,7 @@ extern "C" {
 #define B200MVS_ERR_CANCELLED   (-4)  /* progress.cancelled was set (dmrecon.cc:100-104, RECON_CANCELLED) */
 #define B200MVS_ERR_OVERFLOW    (-5)  /* frontier buffer capacity exceeded                                 */
 #define B200MVS_ERR_UNSUPPORTED (-6)  /* setting outside the range the kernels implement (see below)       */
+#define B200MVS_ERR_NO_MEMORY   (-7)  /* one reference view does not fit the device budget on its own      */
 
 #define B200MVS_MAX_GLOBAL_VIEWS 32   /* settings.global_vs_max must be <= 32 (reference default 20)      */
 #define B200MVS_MAX_LOCAL_VIEWS  4    /* settings.nr_recon_neighbors must be 1..4 (reference default 4)   */
@@ -159,8 +160,9 @@ int b200mvs_upload_view_device(b200mvs_ctx* ctx, int view_id, const uint8_t* rgb
 /* Camera and image size only - SingleView::create (single_view.cc:24-53).  The reference creates a SingleView for every
  * valid view but loads colour images only for the master view and its selected neighbours (dmrecon.cc:78,238-240); a
  * caller that wants the same economy registers all cameras, asks b200mvs_global_view_selection which views are needed
- * and uploads only those images.  b200mvs_reconstruct fails with B200MVS_ERR_INVALID_ARG ("color image of view N is not
- * loaded") when a needed image is missing. */
+ * and uploads only those images - or installs an image source (b200mvs_set_image_source), which loads them on demand.
+ * Without a source b200mvs_reconstruct fails with B200MVS_ERR_INVALID_ARG ("color image of view N is not loaded") when a
+ * needed image is missing. */
 int b200mvs_set_view_camera(b200mvs_ctx* ctx, int view_id, int w, int h, float flen, float paspect,
                             const float ppoint[2], const float rot[9], const float trans[3]);
 /* mve::Bundle::Features (bundle.h:51-60) as position + CSR list of referencing view ids. */
@@ -169,6 +171,7 @@ int b200mvs_set_features(b200mvs_ctx* ctx, int n_features, const float* pos,
 
 /* ---- inspection (parity of the pyramid, image_tools.h:617-694) ---- */
 int b200mvs_num_levels(b200mvs_ctx* ctx, int view_id);
+/* With an image source installed, an evicted view is fetched again (its pyramid is rebuilt bit for bit). */
 int b200mvs_get_level(b200mvs_ctx* ctx, int view_id, int level, int* w, int* h, uint8_t* rgb_host_or_null);
 
 /* ---- DMRecon::analyzeFeatures + globalViewSelection (dmrecon.cc:179-241, global_view_selection.cc) ---- */
@@ -208,10 +211,67 @@ int b200mvs_optimize_patches(b200mvs_ctx* ctx, const b200mvs_settings* s, int re
  * maps: array of n_refs entries, or NULL to leave the results on the device (HBM-resident timing);
  * progress: array of n_refs entries or NULL; stats: one aggregate or NULL.
  * A view whose global view selection is empty makes the call fail with B200MVS_ERR_GLOBAL_VS
- * (failed_view_or_null receives its id). */
+ * (failed_view_or_null receives its id).
+ * With an image source installed (b200mvs_set_image_source) the batch is split into groups that fit the budget
+ * (b200mvs_plan_batches with available = budget - fixed bytes); each group evicts the pyramids it does not need (least
+ * recently used first), fetches the images it lacks and runs its own frontier launch.  A view's maps do not depend on
+ * which views share its launch, so they are bit-identical to one launch of the whole batch.  Across groups `stats` sums
+ * counts and times, takes the maximum of n_entries_peak and counts one patch launch per group; a view cancelled before
+ * its group starts never runs; B200MVS_ERR_CANCELLED is returned only when every view was cancelled; maps == NULL with
+ * more than one group fails with B200MVS_ERR_INVALID_ARG (the results of a group do not stay on the device); a view that
+ * does not fit on its own fails the call with B200MVS_ERR_NO_MEMORY (failed_view_or_null receives its id).  At most 4000
+ * views per group (per call without a source). */
 int b200mvs_reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* ref_views,
                         b200mvs_maps* maps, b200mvs_progress* progress, b200mvs_stats* stats,
                         int32_t* failed_view_or_null);
+
+/* ---- device memory budget: images loaded on demand (ImagePyramidCache::cleanup, image_pyramid.cc:134-155) ----
+ * Without a source (the default) every pyramid stays resident until the context is destroyed and b200mvs_reconstruct runs a
+ * batch in one launch whatever its size. */
+typedef struct b200mvs_image {
+    const uint8_t* rgb;           /* HOST pointer, h x w x channels, row-major; valid until the release callback */
+    int32_t w, h, channels;       /* must equal the size registered for the view; channels 1..4                  */
+} b200mvs_image;
+/* Returns 0 and fills *out with the `undistorted` image of view_id, or non-zero when it cannot be loaded. */
+typedef int  (*b200mvs_fetch_fn)(void* user, int32_t view_id, b200mvs_image* out);
+/* Called once per successful fetch, after the image was copied; the pointer may be freed. */
+typedef void (*b200mvs_release_fn)(void* user, int32_t view_id);
+/* Installs (fetch != NULL) or removes (fetch == NULL) the image source of the context and sets its device budget.
+ * budget_bytes = 0: 90 % of the free bytes cudaMemGetInfo reports at this call.  The budget bounds every device allocation
+ * of the context (accounted in requested bytes); installing it evicts pyramids and drops idle workspace until the resident
+ * bytes fit.  With a source, a view whose pyramid is needed and not resident (b200mvs_reconstruct, b200mvs_get_level,
+ * b200mvs_optimize_patches) is fetched and uploaded, and pyramids - also those the caller uploaded - may be evicted.
+ * The callbacks run on the calling thread WITH THE CONTEXT LOCK HELD: they must not call into this context. */
+int b200mvs_set_image_source(b200mvs_ctx* ctx, b200mvs_fetch_fn fetch, b200mvs_release_fn release, void* user,
+                             uint64_t budget_bytes);
+
+typedef struct b200mvs_memory {
+    uint64_t budget;              /* 0 = no source installed (no limit)                                           */
+    uint64_t fixed;               /* bytes that do not depend on the batch: view table, sRGB table, settings and frontier
+                                     control block, two upload staging buffers of the largest registered image (bound) */
+    uint64_t resident;            /* device bytes the context holds now                                          */
+    uint64_t peak;                /* maximum of `resident` since creation or since the source was installed        */
+    uint64_t n_loads;             /* images fetched through the source                                           */
+    uint64_t bytes_loaded;        /* host bytes of those images                                                  */
+    uint64_t n_evictions;         /* pyramids evicted                                                            */
+    uint64_t n_groups;            /* launches (sub-batches) of the last b200mvs_reconstruct                       */
+} b200mvs_memory;
+int b200mvs_memory_stats(b200mvs_ctx* ctx, b200mvs_memory* out);
+
+/* Device bytes one b200mvs_reconstruct launch of these reference views needs beyond the fixed bytes: the pyramids of the
+ * views and their global selections (every level, 20 bytes per texel at a row pitch of 4 texels), the maps (40 bytes per
+ * pixel of level `scale`, + 2 KiB), the frontier arrays (169 bytes per entry, max(2 x pixels, seeds, 65536) entries), the
+ * tile arrays (12 bytes per 16x16 tile) and the per-view arrays.  b200mvs_reconstruct reserves exactly these sizes.  Works
+ * in a planning context (cameras and features suffice); prepared plans are read, not consumed. */
+int b200mvs_working_set(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* ref_views, uint64_t* bytes);
+
+/* Splits the reference views into groups whose working sets fit `available` bytes; group_of_ref[j] receives the group of
+ * ref_views[j]; returns the number of groups.  Deterministic: a group opens with the first unassigned view in the given
+ * order, then repeatedly takes the unassigned view that fits and adds the fewest new pyramid bytes (ties: lowest index),
+ * until none fits (or the group has 4000 views).  B200MVS_ERR_NO_MEMORY when a view does not fit on its own
+ * (failed_view_or_null receives its id). */
+int b200mvs_plan_batches(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* ref_views,
+                         uint64_t available, int32_t* group_of_ref, int32_t* failed_view_or_null);
 
 /* ---- consumers of the depth maps, on the device (SURVEY.md 8f rank 2 and 3).  Stateless: host buffers in, host buffers
  *      out, `device` = CUDA device ordinal.  Errors: negative code, message from b200mvs_depthmap_last_error(). ---- */

@@ -24,9 +24,10 @@ _LIB = None
 
 
 class B200MVSError(RuntimeError):
-    def __init__(self, code: int, msg: str):
+    def __init__(self, code: int, msg: str, failed_view: int = -1):
         super().__init__("b200mvs error %d: %s" % (code, msg))
         self.code = code
+        self.failed_view = failed_view
 
 
 class Settings(C.Structure):
@@ -79,7 +80,27 @@ EXPORTS = ["b200mvs_default_settings", "b200mvs_create", "b200mvs_destroy", "b20
            "b200mvs_upload_view", "b200mvs_upload_view_device", "b200mvs_set_view_camera", "b200mvs_set_features", "b200mvs_num_levels",
            "b200mvs_get_level", "b200mvs_global_view_selection", "b200mvs_optimize_patches", "b200mvs_reconstruct",
            "b200mvs_plan_views", "b200mvs_set_patch_mode", "b200mvs_depthmap_last_error", "b200mvs_depthmap_confidence_clean",
-           "b200mvs_depthmap_cleanup", "b200mvs_depthmap_triangulate", "b200mvs_depthmap_pointset"]
+           "b200mvs_depthmap_cleanup", "b200mvs_depthmap_triangulate", "b200mvs_depthmap_pointset",
+           "b200mvs_set_image_source", "b200mvs_memory_stats", "b200mvs_working_set", "b200mvs_plan_batches"]
+
+ERR_NO_MEMORY = -7
+
+
+class _Image(C.Structure):
+    _fields_ = [("rgb", C.c_void_p), ("w", C.c_int32), ("h", C.c_int32), ("channels", C.c_int32)]
+
+
+_FETCH_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int32, C.POINTER(_Image))
+_RELEASE_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_int32)
+
+
+class Memory(C.Structure):
+    """b200mvs_memory: device budget and accounting of one context (include/b200mvs.h)."""
+    _fields_ = [("budget", C.c_uint64), ("fixed", C.c_uint64), ("resident", C.c_uint64), ("peak", C.c_uint64),
+                ("n_loads", C.c_uint64), ("bytes_loaded", C.c_uint64), ("n_evictions", C.c_uint64), ("n_groups", C.c_uint64)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
 
 
 def lib():
@@ -112,6 +133,10 @@ def lib():
                                       C.c_void_p]
     L.b200mvs_plan_views.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
     L.b200mvs_set_patch_mode.argtypes = [C.c_void_p, C.c_int, C.c_int64]
+    L.b200mvs_set_image_source.argtypes = [C.c_void_p, _FETCH_FN, _RELEASE_FN, C.c_void_p, C.c_uint64]
+    L.b200mvs_memory_stats.argtypes = [C.c_void_p, C.c_void_p]
+    L.b200mvs_working_set.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+    L.b200mvs_plan_batches.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]
     _LIB = L
     return L
 
@@ -150,13 +175,73 @@ class Scene:
         return rc
 
     @classmethod
-    def from_synth(cls, s, device: int = 0, views: Optional[Sequence[int]] = None) -> "Scene":
-        """Uploads a mve_b200.synth.Scene (host images -> device, pyramids built on the device)."""
+    def from_synth(cls, s, device: int = 0, views: Optional[Sequence[int]] = None, lazy: bool = False,
+                   budget_bytes: int = 0) -> "Scene":
+        """Uploads a mve_b200.synth.Scene (host images -> device, pyramids built on the device).
+        lazy: register cameras only and install an image source over the scene's images (loaded when a call needs them,
+        evicted to stay within budget_bytes; 0 = 90 % of the free device memory)."""
         sc = cls(s.n_views, device)
         for v in (range(s.n_views) if views is None else views):
-            sc.set_view(v, s.images[v], s.flen[v], s.paspect[v], s.ppoint[v], s.rot[v], s.trans[v])
+            if lazy:
+                sc.set_view_camera(v, s.width, s.height, s.flen[v], s.paspect[v], s.ppoint[v], s.rot[v], s.trans[v])
+            else:
+                sc.set_view(v, s.images[v], s.flen[v], s.paspect[v], s.ppoint[v], s.rot[v], s.trans[v])
         sc.set_features(s.feat_pos, s.feat_refs)
+        if lazy:
+            sc.set_image_source(lambda v: s.images[v], budget_bytes)
         return sc
+
+    def set_image_source(self, fetch, budget_bytes: int = 0):
+        """Loads images on demand: fetch(view_id) returns the view's H x W x C uint8 image (the size registered for the view).
+        budget_bytes bounds the device memory of this context (0 = 90 % of the free bytes now); pyramids no running call
+        needs are evicted and fetched again when needed.  fetch=None removes the source."""
+        held = {}
+
+        def _fetch(_user, view_id, out):
+            try:
+                img = np.ascontiguousarray(fetch(int(view_id)), dtype=np.uint8)
+                if img.ndim == 2:
+                    img = img[:, :, None]
+                held[int(view_id)] = img
+                out.contents.rgb = img.ctypes.data
+                out.contents.h, out.contents.w, out.contents.channels = img.shape
+                return 0
+            except Exception:
+                return 1
+
+        def _release(_user, view_id):
+            held.pop(int(view_id), None)
+
+        if fetch is None:
+            self._source = None
+            self._check(self._lib.b200mvs_set_image_source(self._h, _FETCH_FN(), _RELEASE_FN(), None, 0))
+            return
+        cbs = (_FETCH_FN(_fetch), _RELEASE_FN(_release), held)
+        self._check(self._lib.b200mvs_set_image_source(self._h, cbs[0], cbs[1], None, int(budget_bytes)))
+        self._source = cbs                       # the C side keeps the function pointers: keep the ctypes objects alive
+
+    def memory_stats(self) -> Memory:
+        m = Memory()
+        self._check(self._lib.b200mvs_memory_stats(self._h, C.byref(m)))
+        return m
+
+    def working_set(self, settings: Settings, ref_views: Sequence[int]) -> int:
+        """Device bytes one launch of these reference views needs beyond the fixed allocations."""
+        refs = np.asarray(ref_views, np.int32)
+        out = C.c_uint64()
+        self._check(self._lib.b200mvs_working_set(self._h, C.byref(settings), len(refs), _p(refs), C.byref(out)))
+        return out.value
+
+    def plan_batches(self, settings: Settings, ref_views: Sequence[int], available: int):
+        """Groups of these reference views whose working sets fit `available` bytes: (n_groups, group of each view)."""
+        refs = np.asarray(ref_views, np.int32)
+        groups = np.full(len(refs), -1, np.int32)
+        failed = C.c_int32(-1)
+        rc = self._lib.b200mvs_plan_batches(self._h, C.byref(settings), len(refs), _p(refs), int(available), _p(groups),
+                                            C.byref(failed))
+        if rc < 0:
+            raise B200MVSError(rc, self._lib.b200mvs_last_error(self._h).decode(), failed.value)
+        return rc, groups
 
     def set_view(self, view_id: int, image: np.ndarray, flen, paspect, ppoint, rot, trans):
         """mve::View with an `undistorted` uint8 image + mve::CameraInfo (camera.h:23-170)."""
@@ -278,7 +363,7 @@ class Scene:
             msg = self._lib.b200mvs_last_error(self._h).decode()
             if failed.value >= 0:
                 msg += " (view %d)" % failed.value
-            raise B200MVSError(rc, msg)
+            raise B200MVSError(rc, msg, failed.value)
         return results, stats
 
 
