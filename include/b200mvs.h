@@ -212,10 +212,11 @@ int b200mvs_optimize_patches(b200mvs_ctx* ctx, const b200mvs_settings* s, int re
  * progress: array of n_refs entries or NULL; stats: one aggregate or NULL.
  * A view whose global view selection is empty makes the call fail with B200MVS_ERR_GLOBAL_VS
  * (failed_view_or_null receives its id).
- * With an image source installed (b200mvs_set_image_source) the batch is split into groups that fit the budget
- * (b200mvs_plan_batches with available = budget - fixed bytes); each group evicts the pyramids it does not need (least
- * recently used first), fetches the images it lacks and runs its own frontier launch.  A view's maps do not depend on
- * which views share its launch, so they are bit-identical to one launch of the whole batch.  Across groups `stats` sums
+ * The batch is split into groups that fit the device budget (b200mvs_plan_batches with available = budget - fixed bytes;
+ * without an image source there is no budget and the batch is one group); each group evicts the pyramids it does not need
+ * (least recently used first), fetches the images it lacks through the source and runs its own frontier launch.  A view's
+ * maps do not depend on which views share its launch, so they are bit-identical to one launch of the whole batch.
+ * Without a source, a needed image that is not loaded fails the call before anything runs.  Across groups `stats` sums
  * counts and times, takes the maximum of n_entries_peak and counts one patch launch per group; a view cancelled before
  * its group starts never runs; B200MVS_ERR_CANCELLED is returned only when every view was cancelled; maps == NULL with
  * more than one group fails with B200MVS_ERR_INVALID_ARG (the results of a group do not stay on the device); a view that
@@ -226,8 +227,8 @@ int b200mvs_reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs,
                         int32_t* failed_view_or_null);
 
 /* ---- device memory budget: images loaded on demand (ImagePyramidCache::cleanup, image_pyramid.cc:134-155) ----
- * Without a source (the default) every pyramid stays resident until the context is destroyed and b200mvs_reconstruct runs a
- * batch in one launch whatever its size. */
+ * Without a source (the default) the context has no budget: no pyramid is evicted, so every one stays resident until the
+ * context is destroyed, and b200mvs_reconstruct runs a batch of up to 4000 views in one launch. */
 typedef struct b200mvs_image {
     const uint8_t* rgb;           /* HOST pointer, h x w x channels, row-major; valid until the release callback */
     int32_t w, h, channels;       /* must equal the size registered for the view; channels 1..4                  */
