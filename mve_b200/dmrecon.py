@@ -183,7 +183,7 @@ class Scene:
         sc = cls(s.n_views, device)
         for v in (range(s.n_views) if views is None else views):
             if lazy:
-                sc.set_view_camera(v, s.width, s.height, s.flen[v], s.paspect[v], s.ppoint[v], s.rot[v], s.trans[v])
+                sc.set_view_camera(v, *s.size(v), s.flen[v], s.paspect[v], s.ppoint[v], s.rot[v], s.trans[v])
             else:
                 sc.set_view(v, s.images[v], s.flen[v], s.paspect[v], s.ppoint[v], s.rot[v], s.trans[v])
         sc.set_features(s.feat_pos, s.feat_refs)

@@ -13,9 +13,11 @@ Outputs (all under tests/golden/):
   depthmap_ops_ref.npz    libs/mve/depthmap.cc results for tests/test_gpu_depthmap_ops.py
   depthmap_edges_ref.npz  the same at the decision boundaries and edge shapes of tests/test_gpu_depthmap_edges.py
   T0s77_ref.npz           mvs::PatchOptimization results on a scene generated with seed 77
+  T5_*, T6_*              like <S>_* above for the scenes with general cameras (group `cameras`); their patch slices
+                          also keep the patches that sample the zoomed views (T5) or the crops (T6)
   T0_ply_ref.npz          .xf files and PLY headers written by the reference CLI with -p
 
-`python tests/golden/make_golden.py [tiny] [baseline_size] [depthmap_ops] [depthmap_edges] [fresh_scene_patches] [ply]`
+`python tests/golden/make_golden.py [tiny] [cameras] [baseline_size] [depthmap_ops] [depthmap_edges] [fresh_scene_patches] [ply]`
 mints only the named groups (default: all).
 """
 import hashlib
@@ -81,7 +83,9 @@ def mint_gvs_only(name):
         shutil.rmtree(tmp, ignore_errors=True)
 
 
-def mint(name, map_views, n_patches=1500):
+def mint(name, map_views, n_patches=1500, focus=()):
+    """focus: views whose patches are kept beyond the random slice - every traced PatchOptimization that samples one of
+    them, up to 1000."""
     s = synth.make_scene(name)
     synth.save_scene_npz(s, os.path.join(GOLD, "%s_scene.npz" % name))
     s = synth.load_scene_npz(os.path.join(GOLD, "%s_scene.npz" % name))
@@ -110,13 +114,18 @@ def mint(name, map_views, n_patches=1500):
         seeds = np.nonzero(tin["n_local"] == 0)[0]
         rest = np.nonzero(tin["n_local"] != 0)[0]
         rng = np.random.default_rng(7)
-        pick = np.sort(np.concatenate([seeds, rng.choice(rest, size=min(n_patches, len(rest)), replace=False)]))
+        pick = np.concatenate([seeds, rng.choice(rest, size=min(n_patches, len(rest)), replace=False)])
+        if focus:
+            tout = r["trace_out"]
+            near = np.nonzero(np.isin(tin["local_ids"], focus).any(1) | np.isin(tout["local_ids"], focus).any(1))[0]
+            pick = np.concatenate([pick, rng.choice(near, size=min(1000, len(near)), replace=False)])
+        pick = np.unique(pick)
         pin = np.ascontiguousarray(tin[pick])
         # a few hostile inputs: image border, negative depth slope, far-off depth
         extra = np.zeros(6, O.PATCH_IN)
         extra["local_ids"] = -1
         extra[0] = (1, 1, 5.0, 0, 0, 0, [-1] * 4)
-        extra[1] = (s.width // (2 ** s.scale) - 2, 10, 5.0, 0, 0, 0, [-1] * 4)
+        extra[1] = (s.size(ref)[0] // (2 ** s.scale) - 2, 10, 5.0, 0, 0, 0, [-1] * 4)
         extra[2] = (40, 40, 5.0, -3.0, 0.0, 0, [-1] * 4)
         extra[3] = (40, 40, 50.0, 0, 0, 0, [-1] * 4)
         extra[4] = (40, 40, 0.5, 0, 0, 0, [-1] * 4)
@@ -293,7 +302,7 @@ def mint_ply():
 
 
 if __name__ == "__main__":
-    parts = sys.argv[1:] or ["tiny", "baseline_size", "depthmap_ops", "depthmap_edges", "fresh_scene_patches", "ply"]
+    parts = sys.argv[1:] or ["tiny", "cameras", "baseline_size", "depthmap_ops", "depthmap_edges", "fresh_scene_patches", "ply"]
     if "tiny" in parts:
         np.save(os.path.join(GOLD, "srgb2lin.npy"), parse_lut())
         mint("T0", [0, 3])
@@ -301,6 +310,9 @@ if __name__ == "__main__":
         mint("T2", [0])
         mint("T4", [1])
         mint_gvs_only("T3")
+    if "cameras" in parts:
+        mint("T5", [1], focus=(5, 6))
+        mint("T6", [2], focus=(1, 3, 5, 7, 9))
     for p in parts:
-        if p != "tiny":
+        if p not in ("tiny", "cameras"):
             globals()["mint_" + p]()

@@ -106,7 +106,7 @@ def _run(lib, s, osc, ref, gsel, settings, pin, mode=1):
 
 @pytest.mark.parametrize("mode", [1, 2])
 @pytest.mark.parametrize("name,view,kw", [("T0", 0, {}), ("T2", 0, {}), ("T4", 1, {}), ("T0", 2, dict(use_color_scale=0)),
-                                          ("T2", 5, dict(nr_recon_neighbors=3))])
+                                          ("T2", 5, dict(nr_recon_neighbors=3)), ("T5", 1, {}), ("T6", 2, {})])
 def test_kernel_body_on_oracle_trace(emu, name, view, kw, mode):
     """Seeds (full local view selection), propagated patches and - on the orbit scene - view replacements."""
     s = golden_scene(name)

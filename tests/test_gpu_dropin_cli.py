@@ -9,6 +9,7 @@ import tempfile
 import numpy as np
 import pytest
 
+from tests.test_gpu_parity import CLI_CONF_P99
 from tests.util import ROOT, golden_ref, golden_scene, map_stats
 
 pytestmark = pytest.mark.gpu
@@ -16,7 +17,7 @@ CLI = os.path.join(ROOT, "oracle", "_ref", "shim", "dmrecon_b200")
 
 
 @pytest.mark.skipif(not os.path.exists(CLI), reason="oracle/_ref/shim/dmrecon_b200 not built (needs the reference sources at build time)")
-@pytest.mark.parametrize("name,views", [("T0", [0, 3]), ("T1", [4])])
+@pytest.mark.parametrize("name,views", [("T0", [0, 3]), ("T1", [4]), ("T5", [1]), ("T6", [2])])
 def test_cli_writes_reference_layout(name, views):
     from mve_b200 import synth
     s = golden_scene(name)
@@ -36,7 +37,7 @@ def test_cli_writes_reference_layout(name, views):
             iou, rel, both = map_stats(ref["depth_%d" % v], depth[:, :, 0])
             assert iou > 0.99
             assert np.percentile(rel, 50) < 5e-4 and np.percentile(rel, 99) < 5e-3
-            assert np.percentile(np.abs(ref["conf_%d" % v] - conf[:, :, 0])[both], 99) < 2e-2
+            assert np.percentile(np.abs(ref["conf_%d" % v] - conf[:, :, 0])[both], 99) < CLI_CONF_P99.get(name, 2e-2)
             if s.scale:
                 und = [f for f in os.listdir(vd) if f.startswith("undist-L%d" % s.scale)]
                 assert und, "undist-L<s> must be saved for scale != 0 (dmrecon.cc:138-143)"

@@ -41,7 +41,7 @@ def _settings(s, **kw):
             O.default_settings(scale=s.scale, nr_recon_neighbors=s.nr_recon_neighbors, **kw))
 
 
-@pytest.mark.parametrize("name", ["T0", "T1", "T2", "T4"])
+@pytest.mark.parametrize("name", ["T0", "T1", "T2", "T4", "T5", "T6"])
 def test_pyramid_bit_exact(ctx, name):
     s, g, o = ctx(name)
     for v in range(s.n_views):
@@ -52,9 +52,11 @@ def test_pyramid_bit_exact(ctx, name):
         assert (g.level(4, 1) == golden_ref("T1")["undist_4"]).all()     # bytes written by the reference
     if name == "T4":
         assert (g.level(1, 1) == golden_ref("T4")["undist_1"]).all()     # odd dimensions at every level
+    if name == "T6":
+        assert (g.level(2, 1) == golden_ref("T6")["undist_2"]).all()     # 179x180 -> 90x90
 
 
-@pytest.mark.parametrize("name", ["T0", "T1", "T2", "T3", "T4"])
+@pytest.mark.parametrize("name", ["T0", "T1", "T2", "T3", "T4", "T5", "T6"])
 def test_global_view_selection_exact(ctx, name):
     s, g, o = ctx(name)
     ref = golden_ref(name)
@@ -67,7 +69,7 @@ def test_global_view_selection_exact(ctx, name):
 
 
 @pytest.mark.parametrize("mode", [1, 2])
-@pytest.mark.parametrize("name", ["T0", "T1", "T2", "T4"])
+@pytest.mark.parametrize("name", ["T0", "T1", "T2", "T4", "T5", "T6"])
 def test_patches_vs_reference_golden(ctx, name, mode):
     """mvs::PatchOptimization results of the compiled reference (ref_harness) on identical inputs, through both device
     implementations (1: one warp per patch, 2: one thread per patch)."""
@@ -92,7 +94,7 @@ def test_patches_vs_reference_golden(ctx, name, mode):
 
 
 @pytest.mark.parametrize("mode", [1, 2])
-@pytest.mark.parametrize("name,view", [("T0", 0), ("T1", 4), ("T2", 0)])
+@pytest.mark.parametrize("name,view", [("T0", 0), ("T1", 4), ("T2", 0), ("T5", 1), ("T6", 2)])
 def test_patches_vs_oracle_trace(ctx, name, view, mode):
     """Every PatchOptimization of a whole strict-order reconstruction (seeds + queue), replayed as one batch."""
     s, g, o = ctx(name)
@@ -112,7 +114,7 @@ def test_patches_vs_oracle_trace(ctx, name, view, mode):
 
 @pytest.mark.parametrize("name,view,tol", [("T0", 0, (0.995, 2e-3)), ("T0", 3, (0.995, 2e-3)), ("T1", 4, (0.995, 2e-3)),
                                            ("T4", 1, (0.995, 2e-3)),
-                                           ("T2", 0, (0.97, 1e-2))])
+                                           ("T2", 0, (0.97, 1e-2)), ("T5", 1, (0.995, 2e-3)), ("T6", 2, (0.995, 2e-3))])
 @pytest.mark.parametrize("thread_min", [0, 1 << 40])
 def test_maps_vs_oracle_same_schedule(ctx, name, view, tol, thread_min):
     """DMRecon::start on the GPU vs the restatement running the identical frontier schedule; every round through the
@@ -155,7 +157,13 @@ def test_maps_vs_oracle_same_schedule_thresholded(ctx, name, view, band, topk):
     assert int(st.n_rounds) > int(st0.n_rounds)
 
 
-@pytest.mark.parametrize("name,view", [("T0", 0), ("T0", 3), ("T1", 4), ("T4", 1)])
+# confidence p99 against the reference CLI where the processing order alone moves it past 2e-2: on T5 view 1 the oracle
+# running the GPU's frontier schedule is 0.0240 away from the CLI (strict order: 0.0008), and the GPU measured 0.0240 on an
+# H100 (700 W); the other figures of T5 stay within the common bounds (oracle frontier vs CLI: depth rel p99 4.6e-3)
+CLI_CONF_P99 = {"T5": 3e-2}
+
+
+@pytest.mark.parametrize("name,view", [("T0", 0), ("T0", 3), ("T1", 4), ("T4", 1), ("T5", 1), ("T6", 2)])
 def test_maps_vs_reference_cli_golden(ctx, name, view):
     """depth-L<s>/conf-L<s>/dz-L<s> written by the unmodified apps/dmrecon CLI."""
     s, g, o = ctx(name)
@@ -169,7 +177,7 @@ def test_maps_vs_reference_cli_golden(ctx, name, view):
     assert np.percentile(rel, 50) < 5e-4
     assert np.percentile(rel, 99) < 5e-3
     assert rel.max() < 3e-2
-    assert np.percentile(np.abs(ref["conf_%d" % view] - m["conf"])[both], 99) < 2e-2
+    assert np.percentile(np.abs(ref["conf_%d" % view] - m["conf"])[both], 99) < CLI_CONF_P99.get(name, 2e-2)
     assert np.percentile(np.abs(ref["dz_%d" % view] - m["dz"])[both], 99) < 1e-2
 
 

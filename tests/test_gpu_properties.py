@@ -11,20 +11,18 @@ pytestmark = pytest.mark.gpu
 
 
 def _gt_depth(scene, view, scale):
-    """Analytic ground truth: distance along each pixel's ray to the synthetic surface (mve_b200.synth)."""
+    """Analytic ground truth: distance along each pixel's ray to the synthetic surface (mve_b200.synth), through the
+    float64 calibration of the view's pyramid level `scale` (tests/camera_reference.py)."""
     import torch
     from mve_b200 import synth
+    from tests import camera_reference as CR
     cfg = scene.meta
     surf = synth._Surface(cfg["surface"], np.random.default_rng(0))
-    W0, H0 = scene.width, scene.height
-    W, H = W0, H0
-    for _ in range(scale):
-        W, H = (W + 1) // 2, (H + 1) // 2
+    W, H, K = CR.view_levels(scene, view)[scale][:3]
     R = torch.as_tensor(scene.rot[view].astype(np.float64).reshape(3, 3))
     Cc = -(R.T @ torch.as_tensor(scene.trans[view].astype(np.float64)))
-    ax = float(scene.flen[view]) * max(W, H)
     ys, xs = torch.meshgrid(torch.arange(H, dtype=torch.float64), torch.arange(W, dtype=torch.float64), indexing="ij")
-    d = torch.stack([(xs + 0.5 - 0.5 * W) / ax, (ys + 0.5 - 0.5 * H) / ax, torch.ones_like(xs)], -1) @ R
+    d = torch.stack([(xs + 0.5 - K[0, 2]) / K[0, 0], (ys + 0.5 - K[1, 2]) / K[1, 1], torch.ones_like(xs)], -1) @ R
     d = d / d.norm(dim=-1, keepdim=True)
     pts, valid = surf.intersect(Cc, d)
     return (pts - Cc).norm(dim=-1).numpy()

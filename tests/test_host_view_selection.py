@@ -12,12 +12,12 @@ def _planning_scene(s):
     from mve_b200 import dmrecon
     g = dmrecon.Scene(s.n_views, device=-1)
     for v in range(s.n_views):
-        g.set_view_camera(v, s.width, s.height, s.flen[v], s.paspect[v], s.ppoint[v], s.rot[v], s.trans[v])
+        g.set_view_camera(v, *s.size(v), s.flen[v], s.paspect[v], s.ppoint[v], s.rot[v], s.trans[v])
     g.set_features(s.feat_pos, s.feat_refs)
     return g
 
 
-@pytest.mark.parametrize("name", ["T0", "T1", "T2", "T3", "T4"])
+@pytest.mark.parametrize("name", ["T0", "T1", "T2", "T3", "T4", "T5", "T6"])
 def test_global_view_selection_matches_reference(name):
     from mve_b200 import dmrecon
     s = golden_scene(name)

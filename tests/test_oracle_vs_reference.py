@@ -48,7 +48,7 @@ def test_pyramid_bit_exact(osc):
     assert (sc.level(1, s.scale) == golden_ref("T4")["undist_1"]).all()
 
 
-@pytest.mark.parametrize("name", ["T0", "T1", "T2", "T3", "T4"])
+@pytest.mark.parametrize("name", ["T0", "T1", "T2", "T3", "T4", "T5", "T6"])
 def test_global_view_selection_exact(osc, name):
     """Integer result of GlobalViewSelection (global_view_selection.cc:34-101) for default and -n 3."""
     s, sc = osc(name)
@@ -59,7 +59,7 @@ def test_global_view_selection_exact(osc, name):
             assert sc.global_view_selection(st, v) == ref["%s_%d" % (tag, v)].tolist(), (name, tag, v)
 
 
-@pytest.mark.parametrize("name", ["T0", "T1", "T2", "T4"])
+@pytest.mark.parametrize("name", ["T0", "T1", "T2", "T4", "T5", "T6"])
 def test_patch_optimization_vs_reference(osc, name):
     """mvs::PatchOptimization through ref_harness: same inputs -> same view ids, floats within FP noise."""
     s, sc = osc(name)
@@ -83,10 +83,12 @@ def test_patch_optimization_vs_reference(osc, name):
 MAP_TOL = {"T0": dict(iou=0.995, p99=2e-3, mx=2e-2, conf=5e-3, dz=5e-3),
            "T4": dict(iou=0.995, p99=2e-3, mx=2e-2, conf=5e-3, dz=5e-3),   # odd sizes: principal point moves per level
            "T1": dict(iou=0.995, p99=2e-3, mx=2e-2, conf=5e-3, dz=5e-3),
+           "T5": dict(iou=0.995, p99=2e-3, mx=2e-2, conf=5e-3, dz=5e-3),   # general cameras (tests/test_cameras.py)
+           "T6": dict(iou=0.995, p99=2e-3, mx=2e-2, conf=5e-3, dz=5e-3),
            "T2": dict(iou=0.98, p99=1e-2, mx=5e-2, conf=1e-1, dz=1e-2)}
 
 
-@pytest.mark.parametrize("name,views", [("T0", [0, 3]), ("T1", [4]), ("T2", [0]), ("T4", [1])])
+@pytest.mark.parametrize("name,views", [("T0", [0, 3]), ("T1", [4]), ("T2", [0]), ("T4", [1]), ("T5", [1]), ("T6", [2])])
 def test_maps_vs_reference_cli(osc, name, views):
     """Whole depth/conf/dz maps of the unmodified apps/dmrecon CLI vs the restatement in strict priority order."""
     s, sc = osc(name)

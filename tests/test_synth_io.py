@@ -48,3 +48,23 @@ def test_npz_roundtrip():
     assert all((a == b).all() for a, b in zip(s.images, t.images))
     assert (s.rot == t.rot).all() and (s.trans == t.trans).all() and (s.feat_pos == t.feat_pos).all()
     assert all((a == b).all() for a, b in zip(s.feat_refs, t.feat_refs))
+
+
+def test_npz_roundtrip_mixed_sizes():
+    """T6 has views of two sizes: they are stored one by one and each keeps its own size; a scene of one size keeps the
+    stacked `images` array."""
+    s = synth.make_scene("T6")
+    with tempfile.TemporaryDirectory() as tmp:
+        p = os.path.join(tmp, "s.npz")
+        synth.save_scene_npz(s, p)
+        t = synth.load_scene_npz(p)
+        assert "images" not in np.load(p).files
+        synth.save_scene_npz(synth.make_scene("T0"), p)
+        assert "images" in np.load(p).files
+    assert all(a.shape == b.shape and (a == b).all() for a, b in zip(s.images, t.images))
+    assert (s.width, s.height) == (t.width, t.height)
+    assert [s.size(v) for v in range(s.n_views)] == [t.size(v) for v in range(t.n_views)]
+    assert [t.images[v].shape[1::-1] for v in range(t.n_views)] == [t.size(v) for v in range(t.n_views)]
+    assert (s.flen == t.flen).all() and (s.paspect == t.paspect).all() and (s.ppoint == t.ppoint).all()
+    assert (s.rot == t.rot).all() and (s.trans == t.trans).all() and (s.feat_pos == t.feat_pos).all()
+    assert all((a == b).all() for a, b in zip(s.feat_refs, t.feat_refs))
