@@ -187,6 +187,21 @@ int b200mvs_global_view_selection(b200mvs_ctx* ctx, const b200mvs_settings* s, i
  * checked against the oracle. */
 int b200mvs_set_patch_mode(b200mvs_ctx* ctx, int mode, int64_t thread_min);
 
+/* Engine knob (no reference counterpart): the initial frontier capacity of a b200mvs_reconstruct launch,
+ * max(ceil(entries_per_px x reference pixels), seeds, min_entries) entries of 169 device bytes each (default 2.0, 65536).
+ * A smaller capacity shrinks b200mvs_working_set, so
+ * b200mvs_plan_batches fits more views per launch; when a frontier round may not fit, the kernel stops before the round's
+ * pushes, the library grows the frontier arrays to max(2 x capacity, what the round may need) entries (fewer when the budget
+ * allows fewer, never fewer than needed) and resumes the launch where it stopped.  Maps and counters do not depend on the
+ * capacity (n_patch_launches, n_kernel_launches and the times count the resumed launches too).  When the budget cannot hold
+ * what the round needs, the call fails with B200MVS_ERR_OVERFLOW and a message naming both entry counts; the context stays
+ * usable.  entries_per_px in [0, 64]; min_entries at most 2^40 and not 0 together with entries_per_px = 0; else
+ * B200MVS_ERR_INVALID_ARG.  Works in a planning context. */
+int b200mvs_set_frontier_capacity(b200mvs_ctx* ctx, double entries_per_px, uint64_t min_entries);
+/* The frontier of the last b200mvs_reconstruct: initial and final capacity in entries (the largest over its launch groups)
+ * and the number of resumes (summed over its groups).  Any pointer may be NULL. */
+int b200mvs_frontier_info(b200mvs_ctx* ctx, uint64_t* initial_entries, uint64_t* final_entries, uint64_t* n_resumes);
+
 /* Prepares, on host threads, what DMRecon::start computes before its queue runs - analyzeFeatures, globalViewSelection and
  * the seed list of processFeatures (dmrecon.cc:179-292) - for the given reference views, so that a LATER
  * b200mvs_reconstruct of these views (same settings) starts its kernel at once.  May be called from another thread WHILE a
@@ -261,8 +276,9 @@ int b200mvs_memory_stats(b200mvs_ctx* ctx, b200mvs_memory* out);
 
 /* Device bytes one b200mvs_reconstruct launch of these reference views needs beyond the fixed bytes: the pyramids of the
  * views and their global selections (every level, 20 bytes per texel at a row pitch of 4 texels), the maps (40 bytes per
- * pixel of level `scale`, + 2 KiB), the frontier arrays (169 bytes per entry, max(2 x pixels, seeds, 65536) entries), the
- * tile arrays (12 bytes per 16x16 tile) and the per-view arrays.  b200mvs_reconstruct reserves exactly these sizes.  Works
+ * pixel of level `scale`, + 2 KiB), the frontier arrays (169 bytes per entry, the initial capacity of
+ * b200mvs_set_frontier_capacity: max(ceil(2 x pixels), seeds, 65536) entries by default), the tile arrays (12 bytes per
+ * 16x16 tile) and the per-view arrays.  b200mvs_reconstruct reserves exactly these sizes before its first launch.  Works
  * in a planning context (cameras and features suffice); prepared plans are read, not consumed. */
 int b200mvs_working_set(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* ref_views, uint64_t* bytes);
 

@@ -81,8 +81,11 @@ EXPORTS = ["b200mvs_default_settings", "b200mvs_create", "b200mvs_destroy", "b20
            "b200mvs_get_level", "b200mvs_global_view_selection", "b200mvs_optimize_patches", "b200mvs_reconstruct",
            "b200mvs_plan_views", "b200mvs_set_patch_mode", "b200mvs_depthmap_last_error", "b200mvs_depthmap_confidence_clean",
            "b200mvs_depthmap_cleanup", "b200mvs_depthmap_triangulate", "b200mvs_depthmap_pointset",
-           "b200mvs_set_image_source", "b200mvs_memory_stats", "b200mvs_working_set", "b200mvs_plan_batches"]
+           "b200mvs_set_image_source", "b200mvs_memory_stats", "b200mvs_working_set", "b200mvs_plan_batches",
+           "b200mvs_set_frontier_capacity", "b200mvs_frontier_info"]
 
+ERR_INVALID_ARG = -1
+ERR_OVERFLOW = -5
 ERR_NO_MEMORY = -7
 
 
@@ -137,6 +140,8 @@ def lib():
     L.b200mvs_memory_stats.argtypes = [C.c_void_p, C.c_void_p]
     L.b200mvs_working_set.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
     L.b200mvs_plan_batches.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]
+    L.b200mvs_set_frontier_capacity.argtypes = [C.c_void_p, C.c_double, C.c_uint64]
+    L.b200mvs_frontier_info.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     _LIB = L
     return L
 
@@ -298,6 +303,19 @@ class Scene:
     def set_patch_mode(self, mode: int = 0, thread_min: int = -1):
         """Engine knob: 1 = one warp per patch, 2 = one thread per patch, 0 = by size (see include/b200mvs.h)."""
         self._check(self._lib.b200mvs_set_patch_mode(self._h, mode, thread_min))
+
+    def set_frontier_capacity(self, entries_per_px: float = 2.0, min_entries: int = 65536):
+        """Initial frontier capacity of a launch: max(ceil(entries_per_px * pixels), seeds, min_entries) entries; a launch
+        that needs more grows its frontier and resumes (see include/b200mvs.h).  Also sizes working_set / plan_batches."""
+        if min_entries < 0:
+            raise B200MVSError(ERR_INVALID_ARG, "frontier capacity: min_entries must not be negative")
+        self._check(self._lib.b200mvs_set_frontier_capacity(self._h, float(entries_per_px), int(min_entries)))
+
+    def frontier_info(self) -> dict:
+        """Frontier of the last reconstruct(): initial and final capacity in entries, number of resumes."""
+        v = [C.c_uint64() for _ in range(3)]
+        self._check(self._lib.b200mvs_frontier_info(self._h, *(C.byref(x) for x in v)))
+        return dict(initial=v[0].value, final=v[1].value, resumes=v[2].value)
 
     def plan_views(self, settings: Settings, ref_views: Sequence[int]):
         """Global view selection + seed lists of these reference views ahead of their reconstruct() call; safe to call from

@@ -156,6 +156,20 @@ uint64_t device_budget()
     return e ? (uint64_t)std::strtoull(e, nullptr, 10) << 20 : 0;
 }
 
+// Initial frontier capacity of a context: B200MVS_FRONTIER_CAPACITY=<entries_per_px>[,<min_entries>] (include/b200mvs.h),
+// min_entries 65536 when omitted; unset = the library's default.
+void set_frontier_capacity(b200mvs_ctx* ctx)
+{
+    const char* e = std::getenv("B200MVS_FRONTIER_CAPACITY");
+    if (!e) return;
+    char* end = nullptr;
+    const double per_px = std::strtod(e, &end);
+    uint64_t min_entries = 65536;
+    if (end == e) throw std::invalid_argument(std::string("B200MVS_FRONTIER_CAPACITY: not a number: ") + e);
+    if (*end == ',') min_entries = (uint64_t)std::strtoull(end + 1, nullptr, 10);
+    if (b200mvs_set_frontier_capacity(ctx, per_px, min_entries) != 0) throw std::invalid_argument(b200mvs_last_error(ctx));
+}
+
 // Global view selection of one request (dmrecon.cc:211-241), done by the batch leader.  The colour images are loaded by
 // the library through the image source when the batch runs.
 void prepare_request(DeviceCtx& D, Request& r)
@@ -287,6 +301,7 @@ DMRecon::start()
         D.held.clear();
         rc = b200mvs_set_image_source(D.ctx, fetch_image, release_image, &D, device_budget());
         if (rc != 0) throw std::runtime_error(b200mvs_last_error(D.ctx));
+        set_frontier_capacity(D.ctx);
         D.features_set = false;
         D.cameras_set = false;
     }
