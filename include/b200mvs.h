@@ -139,9 +139,9 @@ typedef struct b200mvs_stats {
 #define B200MVS_DEVICE_NONE (-1)
 int  b200mvs_create(int device, int n_views, b200mvs_ctx** out);
 void b200mvs_destroy(b200mvs_ctx* ctx);
-const char* b200mvs_last_error(const b200mvs_ctx* ctx);   /* ctx may be NULL: last create() error of the calling thread;
-                                                              the message of a ctx belongs to the last failing call on it (not
-                                                              synchronised: read it from the thread that got the error code) */
+const char* b200mvs_last_error(const b200mvs_ctx* ctx);   /* the message of the calling thread's last failing call, whichever
+                                                              context it was made on (ctx is not used and may be NULL): read
+                                                              it from the thread that got the error code */
 const char* b200mvs_version(void);
 
 /* ---- inputs ---- */
@@ -210,7 +210,8 @@ int b200mvs_frontier_info(b200mvs_ctx* ctx, uint64_t* initial_entries, uint64_t*
  * (re-uploading the image of a view with an UNCHANGED camera is allowed).  b200mvs_global_view_selection of a planned view
  * returns the plan's selection; b200mvs_reconstruct uses a plan once and drops it; changing a camera or the features drops
  * all plans.  Host threads: up to hardware_concurrency(), or the value of the environment variable B200MVS_HOST_THREADS
- * (several processes sharing one box, one per GPU). */
+ * (several processes sharing one box, one per GPU).  Settings and views are checked as b200mvs_reconstruct checks them,
+ * with the same codes and messages. */
 int b200mvs_plan_views(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* ref_views);
 
 /* ---- batch of independent PatchOptimization runs: ctor + doAutoOptimization + computeConfidence

@@ -8,9 +8,9 @@ import pytest
 from tests.util import golden_ref, golden_scene
 
 
-def _planning_scene(s):
+def _planning_scene(s, n_views=None):
     from mve_b200 import dmrecon
-    g = dmrecon.Scene(s.n_views, device=-1)
+    g = dmrecon.Scene(n_views or s.n_views, device=-1)
     for v in range(s.n_views):
         g.set_view_camera(v, *s.size(v), s.flen[v], s.paspect[v], s.ppoint[v], s.rot[v], s.trans[v])
     g.set_features(s.feat_pos, s.feat_refs)
@@ -60,6 +60,41 @@ def test_planning_context_refuses_compute():
     with pytest.raises(dmrecon.B200MVSError) as e:
         g.global_view_selection(st, 99)
     assert "Master view index out of bounds" in str(e.value)
+
+
+BAD_PLANNING_INPUTS = {          # reference view (None: a view without a camera), settings, code, message
+    "view_99": (99, {}, -1, "Master view index out of bounds"),
+    "view_without_camera": (None, {}, -1, "Invalid master view"),
+    "scale_9": (0, dict(scale=9), -1, "Invalid scale factor"),
+    "filter_width_7": (0, dict(filter_width=7), -6, "filterWidth must be 5"),
+    "nr_recon_neighbors_5": (0, dict(nr_recon_neighbors=5), -6, "nrReconNeighbors must be in 1..4"),
+    "global_vs_max_33": (0, dict(global_vs_max=33), -6, "globalVSMax must be in 1..32"),
+    "frontier_band_2": (0, dict(frontier_band=2.0), -1, "frontier_band must be in [0, 1]"),
+}
+
+
+@pytest.mark.parametrize("case", list(BAD_PLANNING_INPUTS))
+def test_planning_entry_points_reject_the_same_inputs(case):
+    """plan_views, global_view_selection, working_set and plan_batches check settings and reference views alike: each bad
+    input fails all four with the same code and message.  plan_views goes first, so no earlier message can stand in for
+    its own."""
+    from mve_b200 import dmrecon
+    ref, settings, code, message = BAD_PLANNING_INPUTS[case]
+    s = golden_scene("T0")
+    g = _planning_scene(s, n_views=s.n_views + 1)           # the last view has no camera
+    ref = s.n_views if ref is None else ref
+    st = dmrecon.Settings(**{"scale": s.scale, **settings})
+    calls = {"plan_views": lambda: g.plan_views(st, [ref]),
+             "global_view_selection": lambda: g.global_view_selection(st, ref),
+             "working_set": lambda: g.working_set(st, [ref]),
+             "plan_batches": lambda: g.plan_batches(st, [ref], 1 << 40)}
+    got = {}
+    for name, call in calls.items():
+        with pytest.raises(dmrecon.B200MVSError) as e:
+            call()
+        got[name] = (e.value.code, str(e.value))
+    assert len(set(got.values())) == 1, got
+    assert got["plan_views"][0] == code and got["plan_views"][1].startswith("b200mvs error %d: %s" % (code, message)), got
 
 
 def test_plan_views_runs_on_host_threads_without_a_gpu():
