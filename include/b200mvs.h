@@ -320,6 +320,76 @@ int b200mvs_depthmap_pointset(int device, const float* depth, int w, int h, cons
                               uint64_t cap_vertices, uint64_t cap_faces, uint64_t* n_vertices, uint64_t* n_faces,
                               double* device_ms_or_null);
 
+/* ---- the whole-scene point set of apps/scene2pset (scene2pset.cc:247-464) on the device ---- */
+/*
+
+ * A handle collects the point sets of many views: b200mvs_pset_add_view runs the per-view work of
+ * b200mvs_depthmap_pointset on one depth map, then the scene-level filters (fill fraction, bounding box, confidence-scaled
+ * normals, vertex -> pixel map), and appends the surviving points to a point set kept in HOST memory, in the order the
+ * views are added.  b200mvs_pset_clip_masks deletes the points that any silhouette mask marks as background.  The handle's
+ * device memory does not grow with the number of views or points: one view's workspace (kept at the largest view added so
+ * far), plus the masks and one chunk of points during clipping.  Errors: negative code, b200mvs_depthmap_last_error(). */
+typedef struct b200mvs_pset b200mvs_pset;
+typedef struct b200mvs_pset_options {
+    int32_t with_normals;         /* -n: angle-weighted vertex normals                                              */
+    int32_t with_conf;            /* -c: boundary confidences with conf_iterations >= 1 rings (scene2pset uses 4)    */
+    int32_t with_scale;           /* -s: scale values (mean distance to the adjacent vertices times scale_factor)     */
+    int32_t poisson_normals;      /* -p: normal *= confidence; needs with_normals and with_conf                     */
+    int32_t correspondence;       /* -C: keep each vertex' pixel; not with use_aabb, and no mask clipping afterwards */
+    int32_t use_aabb;             /* -b: keep a point when aabb_min <= p <= aabb_max on every axis (both faces kept) */
+    float   aabb_min[3], aabb_max[3];
+    float   min_valid_fraction;   /* -f: > 0 skips views whose fill fraction (in the reference's float sums) is lower */
+    float   scale_factor;         /* -S, 2.5                                                                        */
+    float   dd_factor;            /* mve::geom::DD_FACTOR_DEFAULT = 5                                                */
+    int32_t conf_iterations;      /* 4                                                                              */
+} b200mvs_pset_options;
+/* The fields of mve::CameraInfo a view contributes (libs/mve/camera.h), as b200mvs_set_view_camera takes them. */
+typedef struct b200mvs_pset_camera {
+    float flen, paspect, ppoint[2], rot[9], trans[3];
+} b200mvs_pset_camera;
+typedef struct b200mvs_pset_view {
+    int32_t  added;               /* 0: skipped by min_valid_fraction                                                */
+    float    fraction;            /* the fill fraction as the reference computes it (only when min_valid_fraction > 0) */
+    uint64_t n_points;            /* points this view appended (after the bounding box)                              */
+    uint64_t first_index;         /* index of its first point in the point set                                       */
+} b200mvs_pset_view;
+typedef struct b200mvs_pset_info {
+    uint64_t n_points;            /* points in the set                                                              */
+    uint64_t n_colors;            /* colours in the set: less than n_points when a view had no colour image          */
+    uint64_t n_views;             /* views added (not skipped)                                                      */
+    uint64_t device_bytes;        /* device bytes the handle holds now                                              */
+    uint64_t peak_device_bytes;   /* maximum of device_bytes since creation                                         */
+    double   ms_pointset;         /* device time of the per-view kernels (triangulation, normals, confidences, scales) */
+    double   ms_filter;           /* device time of fill count, bounding box, compaction, normal scaling, pixel map  */
+    double   ms_mask;             /* device time of mask clipping, including the transfers of the chunks              */
+} b200mvs_pset_info;
+/* Correspondence metadata of one added view (scene2pset.cc:50-56). */
+typedef struct b200mvs_pset_corr_view {
+    uint32_t view_id, width, height;
+    uint64_t first_index;
+} b200mvs_pset_corr_view;
+
+int b200mvs_pset_create(int device, const b200mvs_pset_options* options, b200mvs_pset** out);
+void b200mvs_pset_destroy(b200mvs_pset* ps);
+/* One view (scene2pset.cc:284-399): depth map w x h, colour image of the same size with 1-4 channels or NULL, camera.
+ * The view's calibration for the map's size and its camera-to-world matrix are formed as CameraInfo forms them. */
+int b200mvs_pset_add_view(b200mvs_pset* ps, int view_id, const float* depth, int w, int h, const uint8_t* color_or_null,
+                          int color_channels, const b200mvs_pset_camera* cam, b200mvs_pset_view* out_or_null);
+/* Silhouette masks (scene2pset.cc:407-464): n_masks one-channel masks of their own sizes with their cameras.  A point is
+ * deleted when, for any mask, it projects inside the mask (0 <= x < w, 0 <= y < h) onto a 0 byte; a projection that is
+ * NaN counts as outside.  The result does not depend on the order of the masks; num_filtered receives the number of
+ * deleted points.  The per-point lists follow mve::TriangleMesh::delete_vertices: a list is filtered only when it has one
+ * entry per point, so a colour list shorter than the point list (a view without a colour image) is left as it is.
+ * Callable once per handle; no view can be added afterwards. */
+int b200mvs_pset_clip_masks(b200mvs_pset* ps, int n_masks, const uint8_t* const* masks, const int32_t* widths,
+                            const int32_t* heights, const b200mvs_pset_camera* cams, uint64_t* num_filtered);
+int b200mvs_pset_get_info(b200mvs_pset* ps, b200mvs_pset_info* out);
+/* Copies the point set out; NULL skips an array.  vertices / normals 3 floats, colours 4 floats (n_colors of them),
+ * values and confidences 1 float per point.  Normals, values and confidences exist when the options asked for them. */
+int b200mvs_pset_read(b200mvs_pset* ps, float* vertices, float* normals, float* colors, float* values, float* confidences);
+/* With options.correspondence: pixel (x, y) of every point, and one record per added view (n_views of them). */
+int b200mvs_pset_read_correspondence(b200mvs_pset* ps, uint32_t* pixels_xy, b200mvs_pset_corr_view* views);
+
 #ifdef __cplusplus
 }
 #endif

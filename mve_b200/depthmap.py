@@ -1,6 +1,6 @@
 """Host-side mirror of the reference's depth-map consumers over the C ABI (include/b200mvs.h):
 mve::image::depthmap_confidence_clean / depthmap_cleanup and mve::geom::depthmap_triangulate (libs/mve/depthmap.{h,cc}),
-the per-view work of apps/scene2pset.  No CPU fallback: the calls fail without a CUDA device."""
+the per-view work of apps/scene2pset, and (scene_pointset) its whole-scene point set.  No CPU fallback: the calls fail without a CUDA device."""
 from __future__ import annotations
 
 import ctypes as C
@@ -111,3 +111,131 @@ def depthmap_pointset(dm: np.ndarray, invproj: np.ndarray, dd_factor: float = DD
     return dict(vertex_ids=vids, vertices=verts[:n].copy(), colors=None if cols is None else cols[:n].copy(), faces=faces[:nf.value].copy(),
                 normals=None if nrm is None else nrm[:n].copy(), confidences=None if cf is None else cf[:n].copy(),
                 scales=None if sc is None else sc[:n].copy(), device_ms=ms.value)
+
+
+class _PsetOptions(C.Structure):
+    _fields_ = [("with_normals", C.c_int32), ("with_conf", C.c_int32), ("with_scale", C.c_int32), ("poisson_normals", C.c_int32),
+                ("correspondence", C.c_int32), ("use_aabb", C.c_int32), ("aabb_min", C.c_float * 3), ("aabb_max", C.c_float * 3),
+                ("min_valid_fraction", C.c_float), ("scale_factor", C.c_float), ("dd_factor", C.c_float), ("conf_iterations", C.c_int32)]
+
+
+class _PsetCamera(C.Structure):
+    _fields_ = [("flen", C.c_float), ("paspect", C.c_float), ("ppoint", C.c_float * 2), ("rot", C.c_float * 9), ("trans", C.c_float * 3)]
+
+
+class _PsetView(C.Structure):
+    _fields_ = [("added", C.c_int32), ("fraction", C.c_float), ("n_points", C.c_uint64), ("first_index", C.c_uint64)]
+
+
+class _PsetInfo(C.Structure):
+    _fields_ = [("n_points", C.c_uint64), ("n_colors", C.c_uint64), ("n_views", C.c_uint64), ("device_bytes", C.c_uint64),
+                ("peak_device_bytes", C.c_uint64), ("ms_pointset", C.c_double), ("ms_filter", C.c_double), ("ms_mask", C.c_double)]
+
+
+class _PsetCorrView(C.Structure):
+    _fields_ = [("view_id", C.c_uint32), ("width", C.c_uint32), ("height", C.c_uint32), ("first_index", C.c_uint64)]
+
+
+def _pset_lib():
+    L = _lib()
+    if not getattr(L, "_pset_ready", False):
+        L.b200mvs_pset_create.argtypes = [C.c_int, C.POINTER(_PsetOptions), C.POINTER(C.c_void_p)]
+        L.b200mvs_pset_destroy.argtypes = [C.c_void_p]
+        L.b200mvs_pset_destroy.restype = None
+        L.b200mvs_pset_add_view.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.POINTER(_PsetCamera),
+                                            C.POINTER(_PsetView)]
+        L.b200mvs_pset_clip_masks.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
+        L.b200mvs_pset_get_info.argtypes = [C.c_void_p, C.POINTER(_PsetInfo)]
+        L.b200mvs_pset_read.argtypes = [C.c_void_p] + [C.c_void_p] * 5
+        L.b200mvs_pset_read_correspondence.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        L._pset_ready = True
+    return L
+
+
+def _camera(cam) -> _PsetCamera:
+    c = _PsetCamera()
+    c.flen, c.paspect = float(cam["flen"]), float(cam["paspect"])
+    c.ppoint[:] = [float(x) for x in np.asarray(cam["ppoint"], np.float32).reshape(2)]
+    c.rot[:] = [float(x) for x in np.asarray(cam["rot"], np.float32).reshape(9)]
+    c.trans[:] = [float(x) for x in np.asarray(cam["trans"], np.float32).reshape(3)]
+    return c
+
+
+def scene_pointset(views, options=None, masks=None, device: int = 0):
+    """The whole-scene point set of apps/scene2pset (scene2pset.cc:247-464) on the device, through b200mvs_pset_*.
+
+    views: dicts with id, depth [H, W] float32, camera (dict of flen, paspect, ppoint, rot, trans as in mve::CameraInfo) and
+    optionally color [H, W] or [H, W, C] uint8 (None: the view adds no colours), in output order.
+    options: with_normals, with_conf, with_scale, poisson_normals, correspondence, aabb ((min xyz), (max xyz)) or None,
+    min_valid_fraction (0), scale_factor (2.5), dd_factor (5), conf_iterations (4).
+    masks: dicts with mask [H, W] uint8 (one channel) and camera; the points any of them marks 0 are deleted.
+
+    Returns dict(vertices [N, 3], normals [N, 3] or None, colors [M, 4] (M < N when a view had no colour image),
+    values [N] or None, confidences [N] or None, views (per input view: id, added, fraction, n_points, first_index),
+    correspondence (pixels [N, 2] uint32, views [(view_id, width, height, first_index)]) or None, num_filtered,
+    info (peak_device_bytes, device_bytes, ms_pointset, ms_filter, ms_mask))."""
+    o = dict(with_normals=False, with_conf=False, with_scale=False, poisson_normals=False, correspondence=False, aabb=None,
+             min_valid_fraction=0.0, scale_factor=2.5, dd_factor=DD_FACTOR_DEFAULT, conf_iterations=4)
+    o.update(options or {})
+    opt = _PsetOptions()
+    opt.with_normals, opt.with_conf, opt.with_scale = int(o["with_normals"]), int(o["with_conf"]), int(o["with_scale"])
+    opt.poisson_normals, opt.correspondence = int(o["poisson_normals"]), int(o["correspondence"])
+    opt.use_aabb = int(o["aabb"] is not None)
+    if o["aabb"] is not None:
+        opt.aabb_min[:] = [float(np.float32(x)) for x in o["aabb"][0]]
+        opt.aabb_max[:] = [float(np.float32(x)) for x in o["aabb"][1]]
+    opt.min_valid_fraction, opt.scale_factor = float(o["min_valid_fraction"]), float(o["scale_factor"])
+    opt.dd_factor, opt.conf_iterations = float(o["dd_factor"]), int(o["conf_iterations"])
+    L = _pset_lib()
+    h = C.c_void_p()
+    _check(L.b200mvs_pset_create(device, C.byref(opt), C.byref(h)))
+    try:
+        per_view = []
+        for v in views:
+            dm = np.ascontiguousarray(v["depth"], np.float32)
+            col = v.get("color")
+            cch = 0
+            if col is not None:
+                col = np.ascontiguousarray(col, np.uint8)
+                if col.shape[:2] != dm.shape:
+                    raise ValueError("Color image dimension mismatch")
+                cch = 1 if col.ndim == 2 else col.shape[2]
+            r = _PsetView()
+            cam = _camera(v["camera"])
+            _check(L.b200mvs_pset_add_view(h, int(v["id"]), _p(dm), dm.shape[1], dm.shape[0], _p(col), cch, C.byref(cam), C.byref(r)))
+            per_view.append(dict(id=int(v["id"]), added=bool(r.added), fraction=float(r.fraction), n_points=int(r.n_points),
+                                 first_index=int(r.first_index)))
+        num_filtered = 0
+        if masks:
+            ms = [np.ascontiguousarray(m["mask"], np.uint8) for m in masks]
+            if any(m.ndim != 2 for m in ms):
+                raise ValueError("masks must have one channel")
+            ptrs = (C.c_void_p * len(ms))(*[m.ctypes.data for m in ms])
+            ws = np.array([m.shape[1] for m in ms], np.int32)
+            hs = np.array([m.shape[0] for m in ms], np.int32)
+            cams = (_PsetCamera * len(ms))(*[_camera(m["camera"]) for m in masks])
+            nf = C.c_uint64(0)
+            _check(L.b200mvs_pset_clip_masks(h, len(ms), ptrs, _p(ws), _p(hs), cams, C.byref(nf)))
+            num_filtered = int(nf.value)
+        info = _PsetInfo()
+        _check(L.b200mvs_pset_get_info(h, C.byref(info)))
+        n, nc = int(info.n_points), int(info.n_colors)
+        verts = np.empty((n, 3), np.float32)
+        nrm = np.empty((n, 3), np.float32) if o["with_normals"] else None
+        cols = np.empty((nc, 4), np.float32)
+        vals = np.empty(n, np.float32) if o["with_scale"] else None
+        cfs = np.empty(n, np.float32) if o["with_conf"] else None
+        _check(L.b200mvs_pset_read(h, _p(verts), _p(nrm), _p(cols), _p(vals), _p(cfs)))
+        corr = None
+        if o["correspondence"]:
+            pix = np.empty((n, 2), np.uint32)
+            meta = (_PsetCorrView * max(1, int(info.n_views)))()
+            _check(L.b200mvs_pset_read_correspondence(h, _p(pix), meta))
+            corr = dict(pixels=pix, views=[(int(m.view_id), int(m.width), int(m.height), int(m.first_index))
+                                           for m in meta[:int(info.n_views)]])
+        return dict(vertices=verts, normals=nrm, colors=cols, values=vals, confidences=cfs, views=per_view, correspondence=corr,
+                    num_filtered=num_filtered,
+                    info=dict(peak_device_bytes=int(info.peak_device_bytes), device_bytes=int(info.device_bytes),
+                              ms_pointset=info.ms_pointset, ms_filter=info.ms_filter, ms_mask=info.ms_mask))
+    finally:
+        L.b200mvs_pset_destroy(h)
