@@ -721,22 +721,25 @@ __global__ void k_export_rgb(const uchar4* __restrict__ src, int w, int h, int p
 // ------------------------------------------------------------------------------------------------
 // kernels: patch optimisation + frontier
 // ------------------------------------------------------------------------------------------------
-#ifndef OPT_TPB
-#define OPT_TPB 384          // threads per CTA of the patch-optimisation kernels: one CTA per SM shares ONE 64 KB table
-#endif
+// OPT_TPB, the threads per CTA of the patch-optimisation kernels, is set in patch_thread.cuh (it lays out shared memory)
 #ifndef OPT_MIN_BLOCKS
-#define OPT_MIN_BLOCKS 1     // CTAs per SM: registers per thread <= 65536 / (OPT_MIN_BLOCKS * OPT_TPB) = 170; shared memory 151 KB per CTA
+#define OPT_MIN_BLOCKS 1     // CTAs per SM: registers per thread <= 65536 / (OPT_MIN_BLOCKS * OPT_TPB) = 170; shared memory 189 KB per CTA
 #endif
 constexpr int OPT_WARPS = OPT_TPB / 32;
 using PatchT = b200mvs::PatchW;    // one warp per patch (latency: small rounds)
 using PatchT1 = b200mvs::PatchT;   // one thread per patch (throughput: large rounds)
-// dynamic shared memory of the kernels that optimise patches: the lane-replicated sRGB table, then one PatchT1 per thread.
+// dynamic shared memory of the kernels that optimise patches: the lane-replicated sRGB table, then one PatchT1 per thread,
+// then the master-texel table of the PatchT1s (PatchT1::mt_tab).
 // The state of a thread's patch is live across the whole sample loop, which needs every register there is: left to the
 // compiler it is spilled to local memory (~100 slots x 128 B per warp - more than L1 holds, so every reload in the per-view
 // set-up and tear-down was an L2 round trip: 19 % of the kernel's time in ncu's stall samples).  In shared memory a reload
-// costs a fixed ~30 cycles.
+// costs a fixed ~30 cycles.  64 KB + 384 x 232 B + 37.5 KB = 193 024 B: with the 8 B of static shared memory and the 1 KB
+// the system reserves per CTA this is the 196 KB carve-out, which leaves 60 KB of L1 for the texels.  The next carve-out
+// (228 KB, 28 KB of L1) costs far more than any table it could hold: with 75 KB of unused shared memory added to the
+// layout without master texels, the C2 step took 169 ms instead of 117 ms (H100 80GB HBM3, 700 W; DESIGN.md §6).
 constexpr size_t OPT_LUT_BYTES = sizeof(float) * (256 * LUT_STRIDE);
-constexpr size_t OPT_SMEM_BYTES = OPT_LUT_BYTES + (size_t)OPT_TPB * sizeof(PatchT1);
+constexpr size_t OPT_SMEM_BYTES = OPT_LUT_BYTES + (size_t)OPT_TPB * sizeof(PatchT1) + PatchT1::MT_BYTES;
+static_assert(OPT_SMEM_BYTES + 8 + 1024 <= 196 * 1024, "the patch kernels' shared memory must stay within the 196 KB carve-out");
 __device__ __forceinline__ PatchT1& thread_patch(float* smem)
 {
     return reinterpret_cast<PatchT1*>(reinterpret_cast<unsigned char*>(smem) + OPT_LUT_BYTES)[threadIdx.x];
