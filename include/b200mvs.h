@@ -390,6 +390,35 @@ int b200mvs_pset_read(b200mvs_pset* ps, float* vertices, float* normals, float* 
 /* With options.correspondence: pixel (x, y) of every point, and one record per added view (n_views of them). */
 int b200mvs_pset_read_correspondence(b200mvs_pset* ps, uint32_t* pixels_xy, b200mvs_pset_corr_view* views);
 
+/* ---- dmrecon straight into scene2pset: the point sets of a batch of reference views without their maps leaving the device ----
+ * Bit-identical to b200mvs_reconstruct(ctx, s, n_refs, ref_views, maps, progress, stats, failed_view_or_null) followed, for
+ * each j in ref_views order, by b200mvs_pset_add_view(ps, ref_views[j], depth_j, w, h, level_j, 3, &cam_j, &views_out[j]),
+ * where level_j is b200mvs_get_level(ctx, ref_views[j], s->scale, ...) and cam_j the fields the view was registered with
+ * (b200mvs_set_view_camera / b200mvs_upload_view): the same arrays from b200mvs_pset_read / _read_correspondence, the same
+ * n_points, n_colors and n_views, the same per-view records (views_out_or_null: n_refs of them, views skipped by
+ * min_valid_fraction and cancelled views included, both with added = 0).
+ *   - Nothing but the surviving points leaves the device: each view's triangulation and filters run on its depth map where
+ *     the reconstruction left it, with the colours read in place from its pyramid level `scale`.
+ *   - Colours: at scale > 0 the level is what dmrecon saves as undist-L<s> (scene2pset -F<s>).  At scale 0 it is the
+ *     `undistorted` image as uploaded, grey (1 or 2 channels) expanded to r = g = b and alpha dropped; for 1, 2, 3 and
+ *     4 channels that is exactly what depthmap_triangulate makes of the `undistorted` image itself (depthmap.cc:349-364:
+ *     channel 0 is grey below 3 channels, channels 1-2 are green and blue from 3 on, alpha is never read).
+ *   - Points are appended in ref_views order, whatever groups the budget makes; nothing depends on group composition.
+ *   - Memory: during the call the handle's per-view workspace lives on the context's device in the context's budget; every
+ *     group is planned with the workspace of the batch's largest map kept free, so b200mvs_memory.peak stays within the
+ *     budget, and a group's maps are consumed before the next group runs.  The workspace is freed when the call returns.
+ *   - Argument checks, error codes, progress, cancellation, stats, groups and the image source are b200mvs_reconstruct's.
+ *     A view cancelled on its own adds nothing (added = 0); every view cancelled gives B200MVS_ERR_CANCELLED.
+ *   - On any error, and when every view was cancelled, the handle's point set, views and times are unchanged: the points are
+ *     committed only when the whole call succeeds.
+ *   - B200MVS_ERR_INVALID_ARG for a NULL context, a planning context, a NULL handle, a handle on another device than the
+ *     context, and a handle whose masks have been applied (clip masks after this call).
+ * Errors: b200mvs_last_error(). */
+int b200mvs_pset_add_reconstruction(b200mvs_pset* ps, b200mvs_ctx* ctx, const b200mvs_settings* s,
+                                    int n_refs, const int32_t* ref_views,
+                                    b200mvs_progress* progress, b200mvs_stats* stats,
+                                    int32_t* failed_view_or_null, b200mvs_pset_view* views_out_or_null);
+
 #ifdef __cplusplus
 }
 #endif

@@ -4,6 +4,7 @@
 #include "patch_opt.cuh"
 #include "patch_warp.cuh"
 #include "patch_thread.cuh"
+#include "pset_device.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -12,6 +13,7 @@
 #include <cstdio>
 #include <cstring>
 #include <cstdlib>
+#include <functional>
 #include <map>
 #include <chrono>
 #include <ctime>
@@ -2059,7 +2061,7 @@ int plan_groups(b200mvs_ctx* ctx, const b200mvs_settings& s, int n, const int32_
 // max(2 x cap, c.need) entries - fewer when the budget allows fewer, never fewer than c.need - and copies what the resumed
 // round still reads: the carried entries of list[1 - p] and the winners, results and `written` flags of the round.  The
 // dead arrays (the consumed list[p], the other run list) are freed first, so the accounted bytes never exceed the final size.
-int grow_frontier(b200mvs_ctx* ctx, const FrontierCtl& c, FrontierParams& P, size_t& cap)
+int grow_frontier(b200mvs_ctx* ctx, const FrontierCtl& c, FrontierParams& P, size_t& cap, uint64_t reserve)
 {
     const uint64_t need = c.need;
     uint64_t room = UINT64_MAX;
@@ -2068,7 +2070,7 @@ int grow_frontier(b200mvs_ctx* ctx, const FrontierCtl& c, FrontierParams& P, siz
         for (size_t i = 0; i < ctx->views.size(); ++i)
             if (ctx->views[i].d_base && !(i < ctx->pinned.size() && ctx->pinned[i])) evictable += ctx->views[i].bytes;
         const uint64_t limit = ctx->mem.budget + evictable;
-        room = limit > ctx->mem.resident ? limit - ctx->mem.resident : 0;
+        room = limit > ctx->mem.resident + reserve ? limit - ctx->mem.resident - reserve : 0;
     }
     auto extra = [&](uint64_t n) {              // accounted bytes the frontier arrays add at n entries
         uint64_t b = 0;
@@ -2109,12 +2111,21 @@ int grow_frontier(b200mvs_ctx* ctx, const FrontierCtl& c, FrontierParams& P, siz
     return 0;
 }
 
+// Where b200mvs_pset_add_reconstruction sends the maps instead of host buffers.  take(j, job) runs for every view of a group
+// that was not cancelled, right after the group's launch, while the group's maps and pyramids are resident; it may
+// allocate up to bytes(w, h) device bytes for a map of w x h pixels through the accounted allocator, and every group's plan
+// keeps that much free for the largest map of the batch.
+struct MapSink {
+    std::function<uint64_t(int w, int h)> bytes;
+    std::function<int(int j, const JobParams& job)> take;
+};
+
 // One frontier launch over the reference views refs[j], j in js (at most MAX_GROUP_VIEWS): makes room for the pyramids
-// they need within the budget, loads the missing ones, runs.  Accumulates `stats`; marks the views that ended cancelled in
-// `view_cancelled`.
+// they need within the budget (`reserve` bytes kept free for the sink), loads the missing ones, runs.  Accumulates
+// `stats`; marks the views that ended cancelled in `view_cancelled`.
 int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int>& js, const int32_t* refs,
-              const std::vector<HostPlan>& plans, b200mvs_maps* maps, b200mvs_progress* progress, b200mvs_stats* stats,
-              int32_t* failed_view, std::vector<char>& view_cancelled)
+              const std::vector<HostPlan>& plans, b200mvs_maps* maps, const MapSink* sink, uint64_t reserve,
+              b200mvs_progress* progress, b200mvs_stats* stats, int32_t* failed_view, std::vector<char>& view_cancelled)
 {
     // `if (progress.cancelled) return` at the head of every stage (dmrecon.cc:100-104,336): a group whose views were all
     // cancelled before it starts loads nothing and never runs
@@ -2137,7 +2148,7 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
     uint64_t missing = 0;
     for (int v : need) if (!ctx->views[v].has_image) missing += pyramid_bytes(ctx->views[v]);
     const uint64_t fixed = fixed_bytes(ctx);
-    auto over = [&](uint64_t ws) { return fixed + ctx->pyr_resident + missing + ws > budget_limit(ctx); };
+    auto over = [&](uint64_t ws) { return fixed + ctx->pyr_resident + missing + ws + reserve > budget_limit(ctx); };
     if (over(workspace_grown_bytes(ctx, W))) shrink_workspace(ctx, W);
     const uint64_t ws = workspace_grown_bytes(ctx, W);
     while (over(ws) && evict_lru(ctx)) {}
@@ -2288,7 +2299,7 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
         ms_all += ms;
         // a batch whose views are all cancelled is not resumed: it ends cancelled like a kernel that stopped by itself
         if (h_ctl->stop != ST_GROW || mirror->cancel) break;
-        if ((rc = grow_frontier(ctx, *h_ctl, P, cap))) return rc;
+        if ((rc = grow_frontier(ctx, *h_ctl, P, cap, reserve))) return rc;
         ++n_resumes;
         ctx->fr_resumes++;
         P.first_list = h_ctl->resume_p ^ 1;
@@ -2302,14 +2313,18 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
     if (stats) stats->n_seeds_success += ctx->h_counters->count[C_SEED_OK];
 
     // ---- results ----
-    if (maps && !cancelled) {
+    if ((maps || sink) && !cancelled) {
         std::vector<unsigned> hslots;
         for (int k = 0; k < n_refs; ++k) {
             const int j = js[k];
             const size_t np = (size_t)jobs[k].W * jobs[k].H;
-            maps[j].width = jobs[k].W; maps[j].height = jobs[k].H;
+            if (maps) { maps[j].width = jobs[k].W; maps[j].height = jobs[k].H; }
             if (job_cancelled[k]) continue;                  // RECON_CANCELLED: nothing is saved (dmrecon.cc:100-104)
             if (progress) progress[j].status = 4;
+            if (sink) {
+                if ((rc = sink->take(j, jobs[k]))) { if (failed_view) *failed_view = refs[j]; return rc; }
+                continue;
+            }
             if (maps[j].depth) CK(cudaMemcpyAsync(maps[j].depth, jobs[k].depth, np * 4, cudaMemcpyDeviceToHost, st));
             if (maps[j].conf) CK(cudaMemcpyAsync(maps[j].conf, jobs[k].conf, np * 4, cudaMemcpyDeviceToHost, st));
             if (maps[j].dz) CK(cudaMemcpyAsync(maps[j].dz, jobs[k].dz, np * 8, cudaMemcpyDeviceToHost, st));
@@ -2352,24 +2367,20 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
     return 0;
 }
 
-} // namespace
-
-extern "C" {
-
-int b200mvs_reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* refs,
-                        b200mvs_maps* maps, b200mvs_progress* progress, b200mvs_stats* stats, int32_t* failed_view)
+// b200mvs_reconstruct with the context locked and a device: without a sink the maps go to `maps` (NULL: stay on the
+// device, one group only); with one, each view's maps go to the sink after its group's launch and no group plans into
+// the sink's bytes for the largest map of the batch.
+int reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* refs, b200mvs_maps* maps,
+                const MapSink* sink, b200mvs_progress* progress, b200mvs_stats* stats, int32_t* failed_view)
 {
-    if (!ctx) return B200MVS_ERR_INVALID_ARG;
-    std::lock_guard<std::mutex> lk(ctx->mtx);
-    int rc = require_device(ctx);
-    if (rc) return rc;
     // without a budget the whole batch is one launch; with one, the limit applies per group
     if (!ctx->mem.budget && n_refs > MAX_GROUP_VIEWS) return fail(B200MVS_ERR_INVALID_ARG, "b200mvs_reconstruct: bad arguments");
     if (failed_view) *failed_view = -1;
     if (stats) std::memset(stats, 0, sizeof(*stats));
     ctx->fr_initial = ctx->fr_final = ctx->fr_resumes = 0;
     std::vector<HostPlan> plans;
-    if ((rc = plan_batch(ctx, s, n_refs, refs, true, progress, failed_view, plans))) return rc;
+    int rc = plan_batch(ctx, s, n_refs, refs, true, progress, failed_view, plans);
+    if (rc) return rc;
     // an image that is missing and cannot be fetched fails the call before anything runs
     if (!ctx->fetch)
         for (int j = 0; j < n_refs; ++j) {
@@ -2381,22 +2392,77 @@ int b200mvs_reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs,
     CK(cudaSetDevice(ctx->device));
 
     // ---- groups that fit the budget, one frontier launch each ----
+    uint64_t reserve = 0;
+    if (sink)
+        for (int j = 0; j < n_refs; ++j) {
+            const HostLevel& L = ctx->views[refs[j]].lv[s->scale];
+            reserve = std::max(reserve, sink->bytes(L.w, L.h));
+        }
     const uint64_t fixed = fixed_bytes(ctx), limit = budget_limit(ctx);
     std::vector<int> group_of;
-    const int n_groups = plan_groups(ctx, *s, n_refs, refs, plans, limit > fixed ? limit - fixed : 0, group_of, failed_view);
+    const int n_groups = plan_groups(ctx, *s, n_refs, refs, plans, limit > fixed + reserve ? limit - fixed - reserve : 0, group_of, failed_view);
     if (n_groups < 0) return n_groups;
-    if (!maps && n_groups > 1)
+    if (!maps && !sink && n_groups > 1)
         return fail(B200MVS_ERR_INVALID_ARG, "maps == NULL keeps the results on the device, but the budget splits the batch into %d launches", n_groups);
     ctx->mem.n_groups = (uint64_t)n_groups;
     std::vector<char> view_cancelled(n_refs, 0);
     for (int g = 0; g < n_groups; ++g) {
         std::vector<int> js;
         for (int j = 0; j < n_refs; ++j) if (group_of[j] == g) js.push_back(j);
-        if ((rc = run_group(ctx, s, js, refs, plans, maps, progress, stats, failed_view, view_cancelled))) return rc;
+        if ((rc = run_group(ctx, s, js, refs, plans, maps, sink, reserve, progress, stats, failed_view, view_cancelled))) return rc;
     }
     ctx->pinned.clear();
     if (std::all_of(view_cancelled.begin(), view_cancelled.end(), [](char c) { return c != 0; }))
         return fail(B200MVS_ERR_CANCELLED, "reconstruction cancelled");
+    return 0;
+}
+
+} // namespace
+
+extern "C" {
+
+int b200mvs_reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* refs,
+                        b200mvs_maps* maps, b200mvs_progress* progress, b200mvs_stats* stats, int32_t* failed_view)
+{
+    if (!ctx) return B200MVS_ERR_INVALID_ARG;
+    std::lock_guard<std::mutex> lk(ctx->mtx);
+    int rc = require_device(ctx);
+    if (rc) return rc;
+    return reconstruct(ctx, s, n_refs, refs, maps, nullptr, progress, stats, failed_view);
+}
+
+int b200mvs_pset_add_reconstruction(b200mvs_pset* ps, b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* refs,
+                                    b200mvs_progress* progress, b200mvs_stats* stats, int32_t* failed_view, b200mvs_pset_view* views_out)
+{
+    namespace PD = b200mvs_pset_dev;
+    if (!ctx) return fail(B200MVS_ERR_INVALID_ARG, "b200mvs_pset_add_reconstruction: null context");
+    std::lock_guard<std::mutex> lk(ctx->mtx);
+    if (failed_view) *failed_view = -1;
+    if (ctx->device == B200MVS_DEVICE_NONE)
+        return fail(B200MVS_ERR_INVALID_ARG, "b200mvs_pset_add_reconstruction: a planning context (B200MVS_DEVICE_NONE) cannot reconstruct");
+    if (int rc = PD::check(ps, ctx->device)) return fail(rc, "%s", b200mvs_depthmap_last_error());
+    // the handle's workspace lives in the context's budget for the duration of the call
+    const PD::Allocator A{ctx, [](void* c, void** p, size_t n) { return dev_alloc(static_cast<b200mvs_ctx*>(c), p, n); },
+                          [](void* c, void* p, size_t n) { dev_free(static_cast<b200mvs_ctx*>(c), p, n); }};
+    std::vector<PD::Block> blocks(std::max(n_refs, 0));
+    MapSink sink;
+    sink.bytes = [&](int w, int h) { return PD::workspace_bytes(ps, w, h); };
+    sink.take = [&](int j, const JobParams& J) {
+        // the camera the view was registered with: scene2pset forms the calibration from it and the map's size
+        const HostView& v = ctx->views[refs[j]];
+        b200mvs_pset_camera cam;
+        cam.flen = v.flen; cam.paspect = v.paspect; cam.ppoint[0] = v.pp[0]; cam.ppoint[1] = v.pp[1];
+        std::memcpy(cam.rot, v.rot, sizeof(cam.rot));
+        std::memcpy(cam.trans, v.trans, sizeof(cam.trans));
+        const HostLevel& L = v.lv[s->scale];
+        const int rc = PD::extract(ps, refs[j], J.depth, J.W, J.H, L.d_img, L.pitch, cam, blocks[j]);
+        return rc ? fail(rc, "view %d: %s", refs[j], b200mvs_depthmap_last_error()) : 0;
+    };
+    PD::use_allocator(ps, &A);
+    const int rc = reconstruct(ctx, s, n_refs, refs, nullptr, &sink, progress, stats, failed_view);
+    PD::use_allocator(ps, nullptr);
+    if (rc) return rc;
+    PD::commit(ps, blocks, views_out);
     return 0;
 }
 

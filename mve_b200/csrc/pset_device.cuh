@@ -1,0 +1,49 @@
+// The point-set handle's side of b200mvs_pset_add_reconstruction.  b200mvs.cu runs the reconstruction and hands every
+// finished depth map, still on the device, to the handle of depthmap.cu together with the view's pyramid level and camera;
+// the points come back to the host per view and are committed in the caller's view order when the whole call succeeded.
+#pragma once
+#include "../../include/b200mvs.h"
+
+#include <cuda_runtime.h>
+
+#include <cstdint>
+#include <vector>
+
+namespace b200mvs_pset_dev {
+
+// A point list of the handle, or the points of one view before they are committed
+struct Points {
+    std::vector<float> verts, normals, colors, values, confs;
+    std::vector<uint32_t> pix;                                   // correspondence: (x, y) per point
+};
+
+// The points of one reference view, held until the call commits them
+struct Block {
+    b200mvs_pset_view rec = {0, 0.f, 0, 0};          // first_index is set by commit
+    Points pts;
+    uint32_t view_id = 0, width = 0, height = 0;
+    double ms_pointset = 0, ms_filter = 0;
+};
+
+// The device allocator of the handle's workspace while a reconstruction runs: the context's accounted one
+struct Allocator {
+    void* user = nullptr;
+    cudaError_t (*alloc)(void* user, void** p, size_t bytes) = nullptr;
+    void (*free)(void* user, void* p, size_t bytes) = nullptr;
+};
+
+// B200MVS_ERR_INVALID_ARG (message in b200mvs_depthmap_last_error) for a NULL handle, a handle on another device than
+// `device` or one whose masks have been applied
+int check(const b200mvs_pset* ps, int device);
+// Device bytes the handle's workspace holds at most for one map of w x h pixels with a colour image
+uint64_t workspace_bytes(const b200mvs_pset* ps, int w, int h);
+// Frees the workspace, then allocates it through `a` from here on (NULL: cudaMalloc)
+void use_allocator(b200mvs_pset* ps, const Allocator* a);
+// What b200mvs_pset_add_view does with the map and a 3-channel colour image, for a DEVICE depth map (w x h floats) and
+// colours read in place from an RGBX level (uchar4, row pitch `pitch` texels); the points go to `out`, not to the handle
+int extract(b200mvs_pset* ps, int view_id, const float* d_depth, int w, int h, const void* d_rgbx, int pitch,
+            const b200mvs_pset_camera& cam, Block& out);
+// Appends the blocks to the handle in their order; records[j] receives block j's record (records may be NULL)
+void commit(b200mvs_pset* ps, const std::vector<Block>& blocks, b200mvs_pset_view* records);
+
+} // namespace b200mvs_pset_dev

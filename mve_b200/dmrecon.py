@@ -84,11 +84,14 @@ EXPORTS = ["b200mvs_default_settings", "b200mvs_create", "b200mvs_destroy", "b20
            "b200mvs_set_image_source", "b200mvs_memory_stats", "b200mvs_working_set", "b200mvs_plan_batches",
            "b200mvs_set_frontier_capacity", "b200mvs_frontier_info", "b200mvs_pset_create", "b200mvs_pset_destroy",
            "b200mvs_pset_add_view", "b200mvs_pset_clip_masks", "b200mvs_pset_get_info", "b200mvs_pset_read",
-           "b200mvs_pset_read_correspondence"]
+           "b200mvs_pset_read_correspondence", "b200mvs_pset_add_reconstruction"]
 
 ERR_INVALID_ARG = -1
+ERR_GLOBAL_VS = -3
+ERR_CANCELLED = -4
 ERR_OVERFLOW = -5
 ERR_NO_MEMORY = -7
+DEVICE_NONE = -1             # B200MVS_DEVICE_NONE: a planning context (cameras, features, view selection; no images)
 
 
 class _Image(C.Structure):
@@ -385,6 +388,13 @@ class Scene:
                 msg += " (view %d)" % failed.value
             raise B200MVSError(rc, msg, failed.value)
         return results, stats
+
+    def reconstruct_pointset(self, settings: Settings, ref_views: Sequence[int], options=None, masks=None, progress=None):
+        """DMRecon::start for a batch of reference views and scene2pset of their maps, without the maps leaving the device
+        (b200mvs_pset_add_reconstruction).  options / masks: as for mve_b200.depthmap.scene_pointset (the masks are applied
+        after the reconstruction); progress: as for reconstruct().  Returns (the dict of depthmap.scene_pointset, Stats)."""
+        from . import depthmap
+        return depthmap.reconstruct_pointset(self, settings, ref_views, options, masks, progress)
 
 
 class DMRecon:
