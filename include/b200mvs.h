@@ -173,6 +173,10 @@ int b200mvs_set_features(b200mvs_ctx* ctx, int n_features, const float* pos,
 int b200mvs_num_levels(b200mvs_ctx* ctx, int view_id);
 /* With an image source installed, an evicted view is fetched again (its pyramid is rebuilt bit for bit). */
 int b200mvs_get_level(b200mvs_ctx* ctx, int view_id, int level, int* w, int* h, uint8_t* rgb_host_or_null);
+/* The same into DEVICE memory: rgb_dev_or_null receives the h x w x 3 bytes b200mvs_get_level writes (NULL: sizes only).  The
+ * buffer is checked as b200mvs_reconstruct_device checks its maps (any alignment) and the stream rule is the same. */
+int b200mvs_get_level_device(b200mvs_ctx* ctx, int view_id, int level, int* w, int* h, uint8_t* rgb_dev_or_null,
+                             void* cuda_stream);
 
 /* ---- DMRecon::analyzeFeatures + globalViewSelection (dmrecon.cc:179-241, global_view_selection.cc) ---- */
 /* Returns the number of selected views (ids ascending in ids_out) or a negative error. */
@@ -241,6 +245,23 @@ int b200mvs_optimize_patches(b200mvs_ctx* ctx, const b200mvs_settings* s, int re
 int b200mvs_reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* ref_views,
                         b200mvs_maps* maps, b200mvs_progress* progress, b200mvs_stats* stats,
                         int32_t* failed_view_or_null);
+
+/* b200mvs_reconstruct with the maps written into DEVICE memory: every non-NULL pointer of maps_dev[j] is device (or managed)
+ * memory on the context's device, in the layouts of b200mvs_maps; depth is required, the others may be NULL; width/height
+ * are written into the host structs.  Settings and view checks, codes and messages, progress, cancellation (a cancelled
+ * view's buffers are left untouched), stats, groups, the image source and the budget are b200mvs_reconstruct's, and each
+ * group's maps are written right after its launch.
+ *   - Before anything runs, each buffer is checked with cudaPointerGetAttributes: host memory (pinned or pageable), memory
+ *     of another device, a pointer that is not 4-byte aligned and a NULL depth give B200MVS_ERR_INVALID_ARG with a message
+ *     naming the view and the field.  A NULL context, settings or maps_dev is B200MVS_ERR_INVALID_ARG; a planning context
+ *     B200MVS_ERR_CUDA.
+ *   - Streams: the library's work waits for an event recorded on cuda_stream (a cudaStream_t; NULL = the legacy default
+ *     stream) at entry, so the caller may produce or reuse the buffers on its stream just before the call.  The call
+ *     returns when the writes are complete.
+ *   - The buffers are the caller's memory: they are not counted in the context's budget. */
+int b200mvs_reconstruct_device(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* ref_views,
+                               b200mvs_maps* maps_dev, void* cuda_stream, b200mvs_progress* progress, b200mvs_stats* stats,
+                               int32_t* failed_view_or_null);
 
 /* ---- device memory budget: images loaded on demand (ImagePyramidCache::cleanup, image_pyramid.cc:134-155) ----
  * Without a source (the default) the context has no budget: no pyramid is evicted, so every one stays resident until the
@@ -375,6 +396,12 @@ void b200mvs_pset_destroy(b200mvs_pset* ps);
  * The view's calibration for the map's size and its camera-to-world matrix are formed as CameraInfo forms them. */
 int b200mvs_pset_add_view(b200mvs_pset* ps, int view_id, const float* depth, int w, int h, const uint8_t* color_or_null,
                           int color_channels, const b200mvs_pset_camera* cam, b200mvs_pset_view* out_or_null);
+/* The same with the depth map and the colour image in DEVICE memory on the handle's device, checked as
+ * b200mvs_reconstruct_device checks its maps (the colour image at any alignment); the work waits for an event recorded on
+ * cuda_stream (NULL = the legacy default stream) at entry, and the call returns when it is done. */
+int b200mvs_pset_add_view_device(b200mvs_pset* ps, int view_id, const float* depth_dev, int w, int h,
+                                 const uint8_t* color_dev_or_null, int color_channels, const b200mvs_pset_camera* cam,
+                                 void* cuda_stream, b200mvs_pset_view* out_or_null);
 /* Silhouette masks (scene2pset.cc:407-464): n_masks one-channel masks of their own sizes with their cameras.  A point is
  * deleted when, for any mask, it projects inside the mask (0 <= x < w, 0 <= y < h) onto a 0 byte; a projection that is
  * NaN counts as outside.  The result does not depend on the order of the masks; num_filtered receives the number of

@@ -5,6 +5,7 @@
 #include "patch_warp.cuh"
 #include "patch_thread.cuh"
 #include "pset_device.cuh"
+#include "device_buffer.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -718,6 +719,33 @@ __global__ void k_export_rgb(const uchar4* __restrict__ src, int w, int h, int p
     const uchar4 t = src[(size_t)y * pitch + x];
     uint8_t* p = dst + ((size_t)y * w + x) * 3;
     p[0] = t.x; p[1] = t.y; p[2] = t.z;
+}
+
+// The view ids of the four slots of `word` under a job's slot -> id table gview[0, n_global), -1 for an empty slot; returns
+// how many are set.  The host maps, b200mvs_optimize_patches and k_slots_to_ids all map slots through this one function.
+__host__ __device__ inline int slots_to_ids(const int* gview, int n_global, unsigned word, int32_t ids[4])
+{
+    int n = 0;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const unsigned sl = (word >> (8 * k)) & 0xFF;
+        ids[k] = sl < (unsigned)n_global ? gview[sl] : -1;
+        n += ids[k] >= 0;
+    }
+    return n;
+}
+
+// view_ids of one reference view in device memory (b200mvs_reconstruct_device): 4 x int32 per pixel from the job's slot
+// words.  `out` need only be 4-byte aligned; a 16-byte-aligned one is written one pixel per store.
+__global__ void k_slots_to_ids(const JobParams job, int32_t* __restrict__ out, bool aligned16)
+{
+    const size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= (size_t)job.W * job.H) return;
+    int32_t ids[4];
+    slots_to_ids(job.gview, job.n_global, __ldg(job.slots + p), ids);
+    int32_t* o = out + 4 * p;
+    if (aligned16) *reinterpret_cast<int4*>(o) = make_int4(ids[0], ids[1], ids[2], ids[3]);
+    else { o[0] = ids[0]; o[1] = ids[1]; o[2] = ids[2]; o[3] = ids[3]; }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1521,16 +1549,22 @@ unsigned ids_to_slots(const std::vector<int>& gsel, const int32_t* ids, int n, b
     return s;
 }
 
-// The inverse: the view ids of the four slots of `word`, -1 for an empty slot; returns how many are set
-int slots_to_ids(const std::vector<int>& gsel, unsigned word, int32_t ids[4])
+// A caller's buffer of a *_device entry point: device (or managed) memory on the context's device, aligned to `align`
+// bytes.  0, or B200MVS_ERR_INVALID_ARG with a message naming the entry point `fn` and the buffer `what`.
+int check_device_buffer(const char* fn, const std::string& what, const void* p, int device, size_t align)
 {
-    int n = 0;
-    for (int k = 0; k < 4; ++k) {
-        const unsigned sl = (word >> (8 * k)) & 0xFF;
-        ids[k] = sl < gsel.size() ? gsel[sl] : -1;
-        n += ids[k] >= 0;
-    }
-    return n;
+    const std::string why = device_buffer_problem(p, device, align);
+    return why.empty() ? 0 : fail(B200MVS_ERR_INVALID_ARG, "%s: %s %s", fn, what.c_str(), why.c_str());
+}
+
+// The calls of the *_device entry points run on ctx->stream after what the caller enqueued on `cuda_stream` (NULL: the
+// legacy default stream) before the call
+int wait_for_caller(b200mvs_ctx* ctx, void* cuda_stream)
+{
+    const cudaEvent_t ev = get_event(ctx, 3);
+    CK(cudaEventRecord(ev, static_cast<cudaStream_t>(cuda_stream)));
+    CK(cudaStreamWaitEvent(ctx->stream, ev, 0));
+    return 0;
 }
 
 } // namespace
@@ -1755,31 +1789,66 @@ int b200mvs_num_levels(b200mvs_ctx* ctx, int id)
     return (int)ctx->views[id].lv.size();
 }
 
-int b200mvs_get_level(b200mvs_ctx* ctx, int id, int level, int* w, int* h, uint8_t* rgb)
+} // extern "C"
+
+namespace {
+
+// b200mvs_get_level (rgb_dev == nullptr) and b200mvs_get_level_device (rgb == nullptr, with the caller's stream): the size
+// of the level and, when a buffer is given, its packed RGB bytes, written in place into a device buffer or through a
+// staging buffer into a host one
+int get_level(b200mvs_ctx* ctx, int id, int level, int* w, int* h, uint8_t* rgb, uint8_t* rgb_dev, void* cuda_stream)
 {
-    if (!ctx) return B200MVS_ERR_INVALID_ARG;
-    std::lock_guard<std::mutex> lk(ctx->mtx);
     if (id < 0 || id >= (int)ctx->views.size() || !ctx->views[id].valid) return fail(B200MVS_ERR_INVALID_ARG, "invalid view");
     const HostView& v = ctx->views[id];
     if (level < 0 || level >= (int)v.lv.size()) return fail(B200MVS_ERR_INVALID_ARG, "invalid level");
     const HostLevel& L = v.lv[level];
     if (w) *w = L.w;
     if (h) *h = L.h;
-    if (!rgb) return 0;
+    if (!rgb && !rgb_dev) return 0;
     // a planning context has no image and no source: it fails in load_views before any device call
-    if (ctx->device != B200MVS_DEVICE_NONE) CK(cudaSetDevice(ctx->device));
+    int rc = 0;
+    if (ctx->device != B200MVS_DEVICE_NONE) {
+        CK(cudaSetDevice(ctx->device));
+        if (rgb_dev && ((rc = check_device_buffer("b200mvs_get_level_device", "rgb_dev", rgb_dev, ctx->device, 1)) ||
+                        (rc = wait_for_caller(ctx, cuda_stream))))
+            return rc;
+    }
     pin_views(ctx, {id});
-    int rc = load_views(ctx, {id}, nullptr);                 // an evicted view is fetched again through the source
-    if (rc) return rc;
+    if ((rc = load_views(ctx, {id}, nullptr))) return rc;   // an evicted view is fetched again through the source
+    const dim3 grid((L.w + 31) / 32, (L.h + 7) / 8), blk(32, 8);
+    if (rgb_dev) {
+        k_export_rgb<<<grid, blk, 0, ctx->stream>>>(L.d_img, L.w, L.h, L.pitch, rgb_dev);
+        CK(cudaGetLastError());
+        CK(cudaStreamSynchronize(ctx->stream));
+        return 0;
+    }
     uint8_t* d = nullptr;
     const size_t bytes = (size_t)L.w * L.h * 3;
     CK(dev_alloc(ctx, reinterpret_cast<void**>(&d), bytes));
-    k_export_rgb<<<dim3((L.w + 31) / 32, (L.h + 7) / 8), dim3(32, 8), 0, ctx->stream>>>(L.d_img, L.w, L.h, L.pitch, d);
+    k_export_rgb<<<grid, blk, 0, ctx->stream>>>(L.d_img, L.w, L.h, L.pitch, d);
     cudaError_t e = cudaMemcpyAsync(rgb, d, bytes, cudaMemcpyDeviceToHost, ctx->stream);
     cudaStreamSynchronize(ctx->stream);
     dev_free(ctx, d, bytes);
     if (e != cudaSuccess) return fail(B200MVS_ERR_CUDA, "get_level copy: %s", cudaGetErrorString(e));
     return 0;
+}
+
+} // namespace
+
+extern "C" {
+
+int b200mvs_get_level(b200mvs_ctx* ctx, int id, int level, int* w, int* h, uint8_t* rgb)
+{
+    if (!ctx) return B200MVS_ERR_INVALID_ARG;
+    std::lock_guard<std::mutex> lk(ctx->mtx);
+    return get_level(ctx, id, level, w, h, rgb, nullptr, nullptr);
+}
+
+int b200mvs_get_level_device(b200mvs_ctx* ctx, int id, int level, int* w, int* h, uint8_t* rgb_dev, void* cuda_stream)
+{
+    if (!ctx) return B200MVS_ERR_INVALID_ARG;
+    std::lock_guard<std::mutex> lk(ctx->mtx);
+    return get_level(ctx, id, level, w, h, nullptr, rgb_dev, cuda_stream);
 }
 
 int b200mvs_global_view_selection(b200mvs_ctx* ctx, const b200mvs_settings* s, int ref, int32_t* ids_out, int cap)
@@ -1921,7 +1990,7 @@ int b200mvs_optimize_patches(b200mvs_ctx* ctx, const b200mvs_settings* s, int re
         b200mvs_patch_out& o = out[i];
         o.conf = r.conf; o.depth = r.depth; o.dz_i = r.dzI; o.dz_j = r.dzJ;
         o.normal[0] = r.nx; o.normal[1] = r.ny; o.normal[2] = r.nz;
-        o.n_local = slots_to_ids(gsel, r.slots, o.local_ids);
+        o.n_local = slots_to_ids(J.gview, J.n_global, r.slots, o.local_ids);
         o.iterations = r.iterations; o.converged = r.flags & 1; o.opti_success = (r.flags >> 1) & 1;
     }
     if (stats) {
@@ -1946,8 +2015,8 @@ namespace {
 // analyzeFeatures + globalViewSelection + seed list per view (dmrecon.cc:179-292) into plans[j].  A plan prepared ahead
 // (b200mvs_plan_views, possibly while the previous batch was running) is used once and dropped when `consume`, read
 // otherwise.  A view whose selection is empty fails the call.
-int plan_batch(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* refs, bool consume,
-               b200mvs_progress* progress, int32_t* failed_view, std::vector<HostPlan>& plans)
+// The settings and reference views of a batch (failed_view receives the view that fails)
+int check_batch(const b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* refs, int32_t* failed_view)
 {
     int rc = check_settings(s);
     if (rc) return rc;
@@ -1960,6 +2029,14 @@ int plan_batch(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const in
             return fail(B200MVS_ERR_UNSUPPORTED, "reference level larger than 65535 pixels per side");
     }
     if (failed_view) *failed_view = -1;
+    return 0;
+}
+
+int plan_batch(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* refs, bool consume,
+               b200mvs_progress* progress, int32_t* failed_view, std::vector<HostPlan>& plans)
+{
+    int rc = check_batch(ctx, s, n_refs, refs, failed_view);
+    if (rc) return rc;
     plans.assign(n_refs, HostPlan{});
     std::vector<int> todo;
     {
@@ -2111,7 +2188,7 @@ int grow_frontier(b200mvs_ctx* ctx, const FrontierCtl& c, FrontierParams& P, siz
     return 0;
 }
 
-// Where b200mvs_pset_add_reconstruction sends the maps instead of host buffers.  take(j, job) runs for every view of a group
+// Where b200mvs_pset_add_reconstruction and b200mvs_reconstruct_device send the maps instead of host buffers.  take(j, job) runs for every view of a group
 // that was not cancelled, right after the group's launch, while the group's maps and pyramids are resident; it may
 // allocate up to bytes(w, h) device bytes for a map of w x h pixels through the accounted allocator, and every group's plan
 // keeps that much free for the largest map of the batch.
@@ -2333,7 +2410,7 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
                 hslots.resize(np);
                 CK(cudaMemcpyAsync(hslots.data(), jobs[k].slots, np * 4, cudaMemcpyDeviceToHost, st));
                 CK(cudaStreamSynchronize(st));
-                for (size_t p = 0; p < np; ++p) slots_to_ids(plans[j].gsel, hslots[p], maps[j].view_ids + 4 * p);
+                for (size_t p = 0; p < np; ++p) slots_to_ids(jobs[k].gview, jobs[k].n_global, hslots[p], maps[j].view_ids + 4 * p);
             }
         }
     }
@@ -2369,7 +2446,7 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
 
 // b200mvs_reconstruct with the context locked and a device: without a sink the maps go to `maps` (NULL: stay on the
 // device, one group only); with one, each view's maps go to the sink after its group's launch and no group plans into
-// the sink's bytes for the largest map of the batch.
+// the sink's bytes for the largest map of the batch (`maps`, when given, still receives every width and height).
 int reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* refs, b200mvs_maps* maps,
                 const MapSink* sink, b200mvs_progress* progress, b200mvs_stats* stats, int32_t* failed_view)
 {
@@ -2429,6 +2506,49 @@ int b200mvs_reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs,
     int rc = require_device(ctx);
     if (rc) return rc;
     return reconstruct(ctx, s, n_refs, refs, maps, nullptr, progress, stats, failed_view);
+}
+
+int b200mvs_reconstruct_device(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* refs, b200mvs_maps* maps_dev,
+                               void* cuda_stream, b200mvs_progress* progress, b200mvs_stats* stats, int32_t* failed_view)
+{
+    static const char* fn = "b200mvs_reconstruct_device";
+    if (!ctx) return fail(B200MVS_ERR_INVALID_ARG, "%s: null context", fn);
+    std::lock_guard<std::mutex> lk(ctx->mtx);
+    if (!maps_dev) return fail(B200MVS_ERR_INVALID_ARG, "%s: maps_dev is NULL", fn);
+    int rc = check_batch(ctx, s, n_refs, refs, failed_view);
+    if (rc || (rc = require_device(ctx))) return rc;
+    // every buffer is checked before anything runs
+    CK(cudaSetDevice(ctx->device));
+    for (int j = 0; j < n_refs; ++j) {
+        const b200mvs_maps& m = maps_dev[j];
+        auto what = [&](const char* field) { return "maps_dev[" + std::to_string(j) + "]." + field + " (view " + std::to_string(refs[j]) + ")"; };
+        if (!m.depth) return fail(B200MVS_ERR_INVALID_ARG, "%s: %s is NULL", fn, what("depth").c_str());
+        const std::pair<const void*, const char*> bufs[] = {{m.depth, "depth"}, {m.conf, "conf"}, {m.dz, "dz"}, {m.normal, "normal"},
+                                                            {m.view_ids, "view_ids"}};
+        for (const auto& b : bufs)
+            if (b.first && (rc = check_device_buffer(fn, what(b.second), b.first, ctx->device, 4))) return rc;
+    }
+    if ((rc = wait_for_caller(ctx, cuda_stream))) return rc;
+    // each view's maps go straight from the group's map arrays into the caller's buffers, on ctx->stream right after the
+    // group's launch; the caller's buffers are not the context's, so the sink reserves nothing in the budget
+    MapSink sink;
+    sink.bytes = [](int, int) { return (uint64_t)0; };
+    sink.take = [&](int j, const JobParams& J) {
+        const b200mvs_maps& m = maps_dev[j];
+        const size_t np = (size_t)J.W * J.H;
+        const cudaStream_t st = ctx->stream;
+        CK(cudaMemcpyAsync(m.depth, J.depth, np * 4, cudaMemcpyDeviceToDevice, st));
+        if (m.conf) CK(cudaMemcpyAsync(m.conf, J.conf, np * 4, cudaMemcpyDeviceToDevice, st));
+        if (m.dz) CK(cudaMemcpyAsync(m.dz, J.dz, np * 8, cudaMemcpyDeviceToDevice, st));
+        if (m.normal) CK(cudaMemcpyAsync(m.normal, J.normal, np * 12, cudaMemcpyDeviceToDevice, st));
+        if (m.view_ids) {
+            k_slots_to_ids<<<(unsigned)((np + 255) / 256), 256, 0, st>>>(J, m.view_ids, reinterpret_cast<uintptr_t>(m.view_ids) % 16 == 0);
+            CK(cudaGetLastError());
+        }
+        return 0;
+    };
+    // maps_dev also goes in as `maps`, which receives each view's width and height as b200mvs_reconstruct's maps do
+    return reconstruct(ctx, s, n_refs, refs, maps_dev, &sink, progress, stats, failed_view);
 }
 
 int b200mvs_pset_add_reconstruction(b200mvs_pset* ps, b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* refs,

@@ -144,6 +144,8 @@ def _pset_lib():
         L.b200mvs_pset_destroy.restype = None
         L.b200mvs_pset_add_view.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.POINTER(_PsetCamera),
                                             C.POINTER(_PsetView)]
+        L.b200mvs_pset_add_view_device.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                                                   C.POINTER(_PsetCamera), C.c_void_p, C.POINTER(_PsetView)]
         L.b200mvs_pset_clip_masks.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
         L.b200mvs_pset_get_info.argtypes = [C.c_void_p, C.POINTER(_PsetInfo)]
         L.b200mvs_pset_read.argtypes = [C.c_void_p] + [C.c_void_p] * 5
@@ -224,7 +226,9 @@ def scene_pointset(views, options=None, masks=None, device: int = 0):
     """The whole-scene point set of apps/scene2pset (scene2pset.cc:247-464) on the device, through b200mvs_pset_*.
 
     views: dicts with id, depth [H, W] float32, camera (dict of flen, paspect, ppoint, rot, trans as in mve::CameraInfo) and
-    optionally color [H, W] or [H, W, C] uint8 (None: the view adds no colours), in output order.
+    optionally color [H, W] or [H, W, C] uint8 (None: the view adds no colours), in output order.  depth and color may be
+    torch CUDA tensors on `device` (both, or depth alone without colours): such a view is read where it is
+    (b200mvs_pset_add_view_device, after the work of the current stream) and gives the same points as its host copy.
     options: with_normals, with_conf, with_scale, poisson_normals, correspondence, aabb ((min xyz), (max xyz)) or None,
     min_valid_fraction (0), scale_factor (2.5), dd_factor (5), conf_iterations (4).
     masks: dicts with mask [H, W] uint8 (one channel) and camera; the points any of them marks 0 are deleted.
@@ -240,6 +244,9 @@ def scene_pointset(views, options=None, masks=None, device: int = 0):
     try:
         per_view = []
         for v in views:
+            if _is_cuda(v["depth"]):
+                per_view.append(_add_device_view(L, h, v))
+                continue
             dm = np.ascontiguousarray(v["depth"], np.float32)
             col = v.get("color")
             cch = 0
@@ -255,6 +262,34 @@ def scene_pointset(views, options=None, masks=None, device: int = 0):
         return _finish(L, h, o, masks, per_view)
     finally:
         L.b200mvs_pset_destroy(h)
+
+
+def _is_cuda(a):
+    return getattr(a, "is_cuda", False) is True
+
+
+def _add_device_view(L, h, v):
+    """One view of scene_pointset whose depth map (and colour image) are CUDA tensors."""
+    import torch
+    dm = v["depth"].to(torch.float32).contiguous()
+    if dm.dim() != 2:
+        raise ValueError("depth must be H x W")
+    col = v.get("color")
+    cch = 0
+    if col is not None:
+        if not _is_cuda(col):
+            raise ValueError("color must be a CUDA tensor when depth is one")
+        col = col.to(torch.uint8).contiguous()
+        if tuple(col.shape[:2]) != tuple(dm.shape):
+            raise ValueError("Color image dimension mismatch")
+        cch = 1 if col.dim() == 2 else col.shape[2]
+    r = _PsetView()
+    cam = _camera(v["camera"])
+    stream = torch.cuda.current_stream(dm.device).cuda_stream
+    _check(L.b200mvs_pset_add_view_device(h, int(v["id"]), C.c_void_p(dm.data_ptr()), dm.shape[1], dm.shape[0],
+                                          None if col is None else C.c_void_p(col.data_ptr()), cch, C.byref(cam),
+                                          C.c_void_p(stream), C.byref(r)))
+    return _view_record(v["id"], r)
 
 
 def reconstruct_pointset(scene, settings, ref_views, options=None, masks=None, progress=None):

@@ -84,9 +84,11 @@ EXPORTS = ["b200mvs_default_settings", "b200mvs_create", "b200mvs_destroy", "b20
            "b200mvs_set_image_source", "b200mvs_memory_stats", "b200mvs_working_set", "b200mvs_plan_batches",
            "b200mvs_set_frontier_capacity", "b200mvs_frontier_info", "b200mvs_pset_create", "b200mvs_pset_destroy",
            "b200mvs_pset_add_view", "b200mvs_pset_clip_masks", "b200mvs_pset_get_info", "b200mvs_pset_read",
-           "b200mvs_pset_read_correspondence", "b200mvs_pset_add_reconstruction"]
+           "b200mvs_pset_read_correspondence", "b200mvs_pset_add_reconstruction", "b200mvs_reconstruct_device",
+           "b200mvs_get_level_device", "b200mvs_pset_add_view_device"]
 
 ERR_INVALID_ARG = -1
+ERR_CUDA = -2
 ERR_GLOBAL_VS = -3
 ERR_CANCELLED = -4
 ERR_OVERFLOW = -5
@@ -134,11 +136,14 @@ def lib():
     L.b200mvs_set_view_camera.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
     L.b200mvs_num_levels.argtypes = [C.c_void_p, C.c_int]
     L.b200mvs_get_level.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.b200mvs_get_level_device.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.b200mvs_global_view_selection.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
     L.b200mvs_optimize_patches.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int,
                                            C.c_void_p, C.c_void_p]
     L.b200mvs_reconstruct.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p]
+    L.b200mvs_reconstruct_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                             C.c_void_p, C.c_void_p]
     L.b200mvs_plan_views.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
     L.b200mvs_set_patch_mode.argtypes = [C.c_void_p, C.c_int, C.c_int64]
     L.b200mvs_set_image_source.argtypes = [C.c_void_p, _FETCH_FN, _RELEASE_FN, C.c_void_p, C.c_uint64]
@@ -153,6 +158,12 @@ def lib():
 
 def _p(a):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def _torch():
+    """torch, imported only by the calls that return CUDA tensors."""
+    import torch
+    return torch
 
 
 class Scene:
@@ -292,12 +303,26 @@ class Scene:
     def num_levels(self, view_id: int) -> int:
         return self._check(self._lib.b200mvs_num_levels(self._h, view_id))
 
-    def level(self, view_id: int, level: int) -> np.ndarray:
+    def level(self, view_id: int, level: int, on_device: bool = False):
+        """The level's packed RGB bytes, H x W x 3: a numpy array, or with on_device a torch uint8 tensor on cuda:<device>
+        (b200mvs_get_level_device, ordered after the current stream's work)."""
         w, h = C.c_int(), C.c_int()
         self._check(self._lib.b200mvs_get_level(self._h, view_id, level, C.byref(w), C.byref(h), None))
+        if on_device:
+            torch = _torch()
+            out = torch.empty((h.value, w.value, 3), dtype=torch.uint8, device=self._torch_device())
+            stream = torch.cuda.current_stream(out.device).cuda_stream
+            self._check(self._lib.b200mvs_get_level_device(self._h, view_id, level, C.byref(w), C.byref(h),
+                                                           C.c_void_p(out.data_ptr()), C.c_void_p(stream)))
+            return out
         out = np.empty((h.value, w.value, 3), np.uint8)
         self._check(self._lib.b200mvs_get_level(self._h, view_id, level, C.byref(w), C.byref(h), _p(out)))
         return out
+
+    def _torch_device(self):
+        if self.device == DEVICE_NONE:
+            raise B200MVSError(ERR_CUDA, "planning context (B200MVS_DEVICE_NONE): no CUDA device, b200mvs has no CPU fallback")
+        return "cuda:%d" % self.device
 
     def global_view_selection(self, settings: Settings, ref_view: int) -> List[int]:
         """DMRecon::globalViewSelection (dmrecon.cc:211-241)."""
@@ -339,16 +364,24 @@ class Scene:
         return out
 
     def reconstruct(self, settings: Settings, ref_views: Sequence[int], download: bool = True,
-                    want=("depth", "conf", "dz", "normal", "view_ids"), out=None, progress=None):
+                    want=("depth", "conf", "dz", "normal", "view_ids"), out=None, progress=None, on_device: bool = False,
+                    stream=None):
         """DMRecon::start for a batch of reference views. Returns (list of map dicts or None, Stats).
         out: optional list (one dict per view) of preallocated host arrays (e.g. pinned) to receive the maps.
-        progress: optional (Progress * n) array, updated live; setting .cancelled from another thread cancels the run."""
+        progress: optional (Progress * n) array, updated live; setting .cancelled from another thread cancels the run.
+        on_device: the maps as torch CUDA tensors on cuda:<device> (b200mvs_reconstruct_device), without leaving the
+        device: depth, conf [H, W] float32, dz [H, W, 2], normal [H, W, 3] float32, view_ids [H, W, 4] int32.  They are
+        allocated by torch, or taken from `out` (contiguous CUDA tensors of those dtypes, shapes and device, else
+        ValueError).  The call's work is ordered after what `stream` (a torch.cuda.Stream; default: the current stream of
+        the scene's device) has enqueued, and the maps are complete when it returns."""
         refs = np.asarray(ref_views, np.int32)
         n = len(refs)
         stats = Stats()
         failed = C.c_int32(-1)
         maps_arr = None
         results = None
+        if download and on_device:
+            return self._reconstruct_device(settings, refs, want, out, progress, stream)
         if download:
             maps_arr = (_Maps * n)()
             results = []
@@ -382,11 +415,56 @@ class Scene:
                     setattr(maps_arr[j], k, d[k].ctypes.data if k in d else None)
         rc = self._lib.b200mvs_reconstruct(self._h, C.byref(settings), n, _p(refs), maps_arr, progress, C.byref(stats),
                                            C.byref(failed))
+        self._raise(rc, failed)
+        return results, stats
+
+    def _raise(self, rc: int, failed):
         if rc != 0:
             msg = self._lib.b200mvs_last_error(self._h).decode()
             if failed.value >= 0:
                 msg += " (view %d)" % failed.value
             raise B200MVSError(rc, msg, failed.value)
+
+    def _reconstruct_device(self, settings, refs, want, out, progress, stream):
+        n = len(refs)
+        stats = Stats()
+        failed = C.c_int32(-1)
+        maps_arr = (_Maps * max(n, 1))()
+        sizes = []
+        for r in refs:
+            w, h = C.c_int(), C.c_int()
+            if self._lib.b200mvs_get_level(self._h, int(r), settings.scale, C.byref(w), C.byref(h), None) != 0:
+                sizes = None                    # b200mvs_reconstruct_device reports it before it looks at the buffers
+                break
+            sizes.append((h.value, w.value))
+        results = None
+        cuda_stream = None
+        if sizes is not None and self.device != DEVICE_NONE:
+            torch = _torch()
+            dev = torch.device(self._torch_device())
+            layout = dict(depth=((), torch.float32), conf=((), torch.float32), dz=((2,), torch.float32),
+                          normal=((3,), torch.float32), view_ids=((4,), torch.int32))
+            results = []
+            for j, (H, W) in enumerate(sizes):
+                if out is not None:
+                    d = out[j]
+                    for k, a in d.items():
+                        if k not in layout:
+                            raise ValueError("out[%d] has an unknown map %r" % (j, k))
+                        if (not isinstance(a, torch.Tensor) or a.device != dev or a.dtype != layout[k][1]
+                                or tuple(a.shape) != (H, W) + layout[k][0] or not a.is_contiguous()):
+                            raise ValueError("out[%d][%s] must be a contiguous %s tensor of shape %s on %s"
+                                             % (j, k, layout[k][1], (H, W) + layout[k][0], dev))
+                else:
+                    d = {k: torch.empty((H, W) + layout[k][0], dtype=layout[k][1], device=dev)
+                         for k in layout if k == "depth" or k in want}
+                results.append(d)
+                for k in layout:
+                    setattr(maps_arr[j], k, d[k].data_ptr() if k in d else None)
+            cuda_stream = (stream if stream is not None else torch.cuda.current_stream(dev)).cuda_stream
+        rc = self._lib.b200mvs_reconstruct_device(self._h, C.byref(settings), n, _p(refs), maps_arr, C.c_void_p(cuda_stream),
+                                                  progress, C.byref(stats), C.byref(failed))
+        self._raise(rc, failed)
         return results, stats
 
     def reconstruct_pointset(self, settings: Settings, ref_views: Sequence[int], options=None, masks=None, progress=None):
