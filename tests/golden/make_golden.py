@@ -16,8 +16,11 @@ Outputs (all under tests/golden/):
   T5_*, T6_*              like <S>_* above for the scenes with general cameras (group `cameras`); their patch slices
                           also keep the patches that sample the zoomed views (T5) or the crops (T6)
   T0_ply_ref.npz          .xf files and PLY headers written by the reference CLI with -p
+  patch_edges_ref.npz     mvs::PatchOptimization results on the inputs of tests/patch_edges.py that sit on the level
+                          borders, the master border and the level switches: <S>_patch_in / _patch_out / _patch_gvs /
+                          _patch_ref_view for T0, T4, T5, T6 (tests/test_patch_edges_reference.py, test_gpu_patch_edges.py)
 
-`python tests/golden/make_golden.py [tiny] [cameras] [baseline_size] [depthmap_ops] [depthmap_edges] [fresh_scene_patches] [ply]`
+`python tests/golden/make_golden.py [tiny] [cameras] [baseline_size] [depthmap_ops] [depthmap_edges] [fresh_scene_patches] [ply] [patch_edges]`
 mints only the named groups (default: all).
 """
 import hashlib
@@ -283,6 +286,50 @@ def mint_fresh_scene_patches():
     print("fresh scene", len(tin), "patches")
 
 
+# scene -> reference view of the edge cases (the view of the scene's patch slice in <S>_ref.npz)
+EDGE_SCENES = (("T0", 0), ("T4", 1), ("T5", 1), ("T6", 2))
+
+
+def save_npz_stable(path, **arrays):
+    """np.savez_compressed with fixed member timestamps, so that a second run writes the same bytes."""
+    import io
+    import zipfile
+    with zipfile.ZipFile(path, "w", zipfile.ZIP_DEFLATED) as z:
+        for k in sorted(arrays):
+            buf = io.BytesIO()
+            np.lib.format.write_array(buf, np.asanyarray(arrays[k]), allow_pickle=False)
+            z.writestr(zipfile.ZipInfo(k + ".npy", date_time=(1980, 1, 1, 0, 0, 0)), buf.getvalue(),
+                       compress_type=zipfile.ZIP_DEFLATED)
+
+
+def mint_patch_edges():
+    """mvs::PatchOptimization through ref_harness on the edge cases of tests/patch_edges.py.make_cases, built from the
+    oracle's execution trace of each scene's reference view (seeded: a second run gives the same bytes)."""
+    from tests import patch_edges as PE
+    data = {}
+    for name, ref in EDGE_SCENES:
+        s = synth.load_scene_npz(os.path.join(GOLD, "%s_scene.npz" % name))
+        osc = O.OracleScene(s)
+        st = O.default_settings(scale=s.scale, nr_recon_neighbors=s.nr_recon_neighbors)
+        gsel = osc.global_view_selection(st, ref)
+        r = osc.reconstruct(st, ref, trace_cap=200000)
+        pin = PE.make_cases(s, ref, s.scale, gsel, r["trace_in"], r["trace_out"], np.random.default_rng(11))
+        with tempfile.TemporaryDirectory(prefix="golden_") as tmp:
+            synth.write_mve_scene(s, tmp)
+            fin, fout = os.path.join(tmp, "pin.bin"), os.path.join(tmp, "pout.bin")
+            pin.tofile(fin)
+            txt = subprocess.run([os.path.join(REF, "ref_harness"), "patches", tmp, str(ref), str(s.scale),
+                                  str(s.nr_recon_neighbors), fin, fout], capture_output=True, text=True, check=True).stdout
+            m = re.search(r"Global View Selection:([ 0-9]*)", txt)
+            data[name + "_patch_gvs"] = np.asarray([int(x) for x in m.group(1).split()], np.int32)
+            data[name + "_patch_out"] = np.fromfile(fout, dtype=O.PATCH_OUT)
+        assert data[name + "_patch_gvs"].tolist() == gsel
+        data[name + "_patch_in"] = pin
+        data[name + "_patch_ref_view"] = np.int32(ref)
+        print(name, "edge patches", len(pin), "reference successes", int((data[name + "_patch_out"]["conf"] > 0).sum()))
+    save_npz_stable(os.path.join(GOLD, "patch_edges_ref.npz"), **data)
+
+
 def mint_ply():
     """.xf files and PLY header / element counts written by the reference CLI with -p (tests/test_gpu_dropin_cli.py)."""
     from tests.test_gpu_dropin_cli import PLY_VIEWS, ply_cmd, read_ply_header
@@ -302,7 +349,8 @@ def mint_ply():
 
 
 if __name__ == "__main__":
-    parts = sys.argv[1:] or ["tiny", "cameras", "baseline_size", "depthmap_ops", "depthmap_edges", "fresh_scene_patches", "ply"]
+    parts = sys.argv[1:] or ["tiny", "cameras", "baseline_size", "depthmap_ops", "depthmap_edges", "fresh_scene_patches", "ply",
+                              "patch_edges"]
     if "tiny" in parts:
         np.save(os.path.join(GOLD, "srgb2lin.npy"), parse_lut())
         mint("T0", [0, 3])
