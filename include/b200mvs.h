@@ -218,6 +218,25 @@ int b200mvs_frontier_info(b200mvs_ctx* ctx, uint64_t* initial_entries, uint64_t*
  * with the same codes and messages. */
 int b200mvs_plan_views(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* ref_views);
 
+/* How the last b200mvs_reconstruct, b200mvs_reconstruct_device or b200mvs_pset_add_reconstruction planned its views
+ * (analyzeFeatures, globalViewSelection and the seed list).  A view with a plan from b200mvs_plan_views uses it; the others
+ * are planned on the device, one CTA per view and one launch per chunk of views that fits the budget, with selections and
+ * seeds equal to the host planner's.  A view is planned on host threads instead when its planning workspace does not fit
+ * the budget on its own, or when min_parallax is above about 41 degrees (the device's table of parallax factors would
+ * exceed 2^22 entries).  The planning allocations go through the budget and are freed before the first launch group, so
+ * they never add to b200mvs_memory.fixed. */
+typedef struct b200mvs_plan_info {
+    uint64_t n_prepared;     /* views taken from b200mvs_plan_views plans */
+    uint64_t n_device;       /* views planned on the device               */
+    uint64_t n_host;         /* views planned on host threads             */
+    double   ms_plan;        /* wall time of the call's planning phase    */
+    double   ms_device;      /* CUDA-event time of the planning kernels   */
+    uint64_t peak_bytes;     /* largest planning allocation               */
+} b200mvs_plan_info;
+/* The b200mvs_plan_info of the last reconstruction (all zero before the first one).  The struct and the function cannot share
+ * one name in C, so the query is named like b200mvs_memory_stats. */
+int b200mvs_plan_stats(b200mvs_ctx* ctx, b200mvs_plan_info* out);
+
 /* ---- batch of independent PatchOptimization runs: ctor + doAutoOptimization + computeConfidence
  *      (patch_optimization.cc:21-242); the patch-level parity entry ---- */
 int b200mvs_optimize_patches(b200mvs_ctx* ctx, const b200mvs_settings* s, int ref_view,
@@ -227,7 +246,8 @@ int b200mvs_optimize_patches(b200mvs_ctx* ctx, const b200mvs_settings* s, int re
 
 /* ---- DMRecon::start (dmrecon.cc:90-172) for a batch of reference views ----
  * Runs analyzeFeatures, globalViewSelection, processFeatures and processQueue for every view in
- * ref_views; all of them advance together, one frontier round per kernel sequence.
+ * ref_views; all of them advance together, one frontier round per kernel sequence.  Views without a b200mvs_plan_views
+ * plan are planned on the device before the first group (b200mvs_plan_info).
  * maps: array of n_refs entries, or NULL to leave the results on the device (HBM-resident timing);
  * progress: array of n_refs entries or NULL; stats: one aggregate or NULL.
  * A view whose global view selection is empty makes the call fail with B200MVS_ERR_GLOBAL_VS
@@ -249,7 +269,8 @@ int b200mvs_reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs,
 /* b200mvs_reconstruct with the maps written into DEVICE memory: every non-NULL pointer of maps_dev[j] is device (or managed)
  * memory on the context's device, in the layouts of b200mvs_maps; depth is required, the others may be NULL; width/height
  * are written into the host structs.  Settings and view checks, codes and messages, progress, cancellation (a cancelled
- * view's buffers are left untouched), stats, groups, the image source and the budget are b200mvs_reconstruct's, and each
+ * view's buffers are left untouched), stats, groups, planning on the device (b200mvs_plan_info), the image source and the
+ * budget are b200mvs_reconstruct's, and each
  * group's maps are written right after its launch.
  *   - Before anything runs, each buffer is checked with cudaPointerGetAttributes: host memory (pinned or pageable), memory
  *     of another device, a pointer that is not 4-byte aligned and a NULL depth give B200MVS_ERR_INVALID_ARG with a message
@@ -434,7 +455,8 @@ int b200mvs_pset_read_correspondence(b200mvs_pset* ps, uint32_t* pixels_xy, b200
  *   - Memory: during the call the handle's per-view workspace lives on the context's device in the context's budget; every
  *     group is planned with the workspace of the batch's largest map kept free, so b200mvs_memory.peak stays within the
  *     budget, and a group's maps are consumed before the next group runs.  The workspace is freed when the call returns.
- *   - Argument checks, error codes, progress, cancellation, stats, groups and the image source are b200mvs_reconstruct's.
+ *   - Argument checks, error codes, progress, cancellation, stats, groups, planning on the device (b200mvs_plan_info) and
+ *     the image source are b200mvs_reconstruct's.
  *     A view cancelled on its own adds nothing (added = 0); every view cancelled gives B200MVS_ERR_CANCELLED.
  *   - On any error, and when every view was cancelled, the handle's point set, views and times are unchanged: the points are
  *     committed only when the whole call succeeds.

@@ -82,7 +82,7 @@ EXPORTS = ["b200mvs_default_settings", "b200mvs_create", "b200mvs_destroy", "b20
            "b200mvs_plan_views", "b200mvs_set_patch_mode", "b200mvs_depthmap_last_error", "b200mvs_depthmap_confidence_clean",
            "b200mvs_depthmap_cleanup", "b200mvs_depthmap_triangulate", "b200mvs_depthmap_pointset",
            "b200mvs_set_image_source", "b200mvs_memory_stats", "b200mvs_working_set", "b200mvs_plan_batches",
-           "b200mvs_set_frontier_capacity", "b200mvs_frontier_info", "b200mvs_pset_create", "b200mvs_pset_destroy",
+           "b200mvs_set_frontier_capacity", "b200mvs_frontier_info", "b200mvs_plan_stats", "b200mvs_pset_create", "b200mvs_pset_destroy",
            "b200mvs_pset_add_view", "b200mvs_pset_clip_masks", "b200mvs_pset_get_info", "b200mvs_pset_read",
            "b200mvs_pset_read_correspondence", "b200mvs_pset_add_reconstruction", "b200mvs_reconstruct_device",
            "b200mvs_get_level_device", "b200mvs_pset_add_view_device"]
@@ -108,6 +108,15 @@ class Memory(C.Structure):
     """b200mvs_memory: device budget and accounting of one context (include/b200mvs.h)."""
     _fields_ = [("budget", C.c_uint64), ("fixed", C.c_uint64), ("resident", C.c_uint64), ("peak", C.c_uint64),
                 ("n_loads", C.c_uint64), ("bytes_loaded", C.c_uint64), ("n_evictions", C.c_uint64), ("n_groups", C.c_uint64)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+class PlanInfo(C.Structure):
+    """b200mvs_plan_info: how the last reconstruction planned its views (include/b200mvs.h)."""
+    _fields_ = [("n_prepared", C.c_uint64), ("n_device", C.c_uint64), ("n_host", C.c_uint64), ("ms_plan", C.c_double),
+                ("ms_device", C.c_double), ("peak_bytes", C.c_uint64)]
 
     def as_dict(self):
         return {k: getattr(self, k) for k, _ in self._fields_}
@@ -152,6 +161,7 @@ def lib():
     L.b200mvs_plan_batches.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]
     L.b200mvs_set_frontier_capacity.argtypes = [C.c_void_p, C.c_double, C.c_uint64]
     L.b200mvs_frontier_info.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.b200mvs_plan_stats.argtypes = [C.c_void_p, C.c_void_p]
     _LIB = L
     return L
 
@@ -346,6 +356,14 @@ class Scene:
         v = [C.c_uint64() for _ in range(3)]
         self._check(self._lib.b200mvs_frontier_info(self._h, *(C.byref(x) for x in v)))
         return dict(initial=v[0].value, final=v[1].value, resumes=v[2].value)
+
+    def plan_info(self) -> dict:
+        """How the last reconstruct(), reconstruct(on_device=True) or reconstruct_pointset() planned its views: prepared by
+        plan_views(), on the device or on host threads, with the planning phase's wall and kernel times and its largest
+        device allocation."""
+        p = PlanInfo()
+        self._check(self._lib.b200mvs_plan_stats(self._h, C.byref(p)))
+        return p.as_dict()
 
     def plan_views(self, settings: Settings, ref_views: Sequence[int]):
         """Global view selection + seed lists of these reference views ahead of their reconstruct() call; safe to call from
