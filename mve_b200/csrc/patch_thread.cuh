@@ -19,7 +19,8 @@
 //                                           sum(n n) = sum(y^2) + p (2 sum(y) + 25 p)
 //       Gauss-Newton, depth only (:283-288) sum_ch cs (sum(d m) - cs sum(d n)) / sum_ch cs^2 sum(d d), with the current
 //                                           scale or the one just updated;
-//     only the normal equations (:324-343, one state in five) are formed per sample, channels first: with q = sum_ch (cs d)^2
+//     only the normal equations (:324-343, read by one state in five) are summed per sample, channels first (by every
+//     lane, without a branch - nearly every warp holds a lane that reads them): with q = sum_ch (cs d)^2
 //     and s = sum_ch cs d (m - cs n) a sample adds (1, di, dj)^T (1, di, dj) q and (1, di, dj) s, whose (1, 1) / first
 //     entries are the depth-only denominator / numerator above.  Only a view replacement (colour scale AND normal step at
 //     one state, rare) sweeps a view twice;
@@ -246,9 +247,10 @@ struct PatchT : PatchState {
         unsigned qpitch;
         float pv0, pv1, pv2;       // NCC pivots
         float c0, c1, c2;          // colour scales (normal equations)
-        bool nrm;                  // form the normal equations
         // Every lane accumulates the same sums, whatever it derives from them after the sweep (the lanes of a warp are at
-        // different states, and sums a lane would skip are still paid by the warp as divergent or predicated code).
+        // different states, and sums a lane would skip are still paid by the warp as divergent or predicated code).  That
+        // includes the normal equations: nearly every warp holds a lane that forms them, so a per-lane branch around them
+        // saved nothing and only split the loop body; a lane that does not form them never reads them.
         // Per channel, with y = n - p around the NCC pivot p = meanX * masterMeanCol:
         //   Sy = sum(y), Syy = sum(y^2), Smy = sum(m y)      -> NCC and colour scale (sum(m n), sum(n n))
         //   Sdm = sum(d m), Sdn = sum(d n), Sdd = sum(d^2)   -> Gauss-Newton numerator / denominator for any scale
@@ -329,7 +331,7 @@ struct PatchT : PatchState {
             Sdma = fma_rn(d[0], m[0], Sdma); Sdmb = fma_rn(d[1], m[1], Sdmb); Sdmc = fma_rn(d[2], m[2], Sdmc);
             Sdna = fma_rn(d[0], n[0], Sdna); Sdnb = fma_rn(d[1], n[1], Sdnb); Sdnc = fma_rn(d[2], n[2], Sdnc);
             Sdda = fma_rn(d[0], d[0], Sdda); Sddb = fma_rn(d[1], d[1], Sddb); Sddc = fma_rn(d[2], d[2], Sddc);
-            if (nrm) {
+            {
                 // patch_optimization.cc:324-343: the rows of a sample are (1, ii, jj) * cs * deriv per channel, so its
                 // products are (1, ii, jj)^T (1, ii, jj) * q and (1, ii, jj) * s with q = sum (cs d)^2 and
                 // s = sum cs d (m - cs n) over the channels
@@ -437,15 +439,14 @@ struct PatchT : PatchState {
                 sw.Wax = Wax; sw.Way = Way; sw.Waz = Waz; sw.Wbx = Wbx; sw.Wby = Wby; sw.Wbz = Wbz;
                 sw.Lax = Lax; sw.Lay = Lay; sw.Lcx = Lcx; sw.Lcy = Lcy; sw.wm1 = wm1; sw.hm1 = hm1; sw.step = step; sw.dd = dd;
                 sw.quad = Lquad; sw.qpitch = (unsigned)Lpitch;
-                sw.pv0 = pv0; sw.pv1 = pv1; sw.pv2 = pv2; sw.c0 = c0; sw.c1 = c1; sw.c2 = c2; sw.nrm = nrm;
+                sw.pv0 = pv0; sw.pv1 = pv1; sw.pv2 = pv2; sw.c0 = c0; sw.c1 = c1; sw.c2 = c2;
                 sw.clear();
                 // The sample loop is software-pipelined two samples deep.  Two slots take turns: as soon as sample k has
                 // been processed, sample k+2 is staged (geometry, quad and master loads) into the slot k was read from, so
                 // its loads have all of sample k+1 to arrive.  The rotation is in the code - the loop is unrolled by two -
                 // and no staged value is copied.  Samples 0..21 run in the loop and 22..24 after it, where only sample 24
-                // is still staged: nothing past the last sample is ever staged.  All 25 samples run, without a branch
-                // except the per-lane normal equations; `ok` collects their validity, and a view with an invalid sample
-                // fails (its sums are never read).
+                // is still staged: nothing past the last sample is ever staged.  All 25 samples run, without a branch;
+                // `ok` collects their validity, and a view with an invalid sample fails (its sums are never read).
                 Staged sa, sb;
                 bool ok = sw.stage(0, sa);
                 ok &= sw.stage(1, sb);
