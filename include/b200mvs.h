@@ -368,9 +368,11 @@ int b200mvs_depthmap_pointset(int device, const float* depth, int w, int h, cons
  * A handle collects the point sets of many views: b200mvs_pset_add_view runs the per-view work of
  * b200mvs_depthmap_pointset on one depth map, then the scene-level filters (fill fraction, bounding box, confidence-scaled
  * normals, vertex -> pixel map), and appends the surviving points to a point set kept in HOST memory, in the order the
- * views are added.  b200mvs_pset_clip_masks deletes the points that any silhouette mask marks as background.  The handle's
- * device memory does not grow with the number of views or points: one view's workspace (kept at the largest view added so
- * far), plus the masks and one chunk of points during clipping.  Errors: negative code, b200mvs_depthmap_last_error(). */
+ * views are added.  b200mvs_pset_clip_masks deletes the points that any silhouette mask marks as background.  The device
+ * memory of a handle made by b200mvs_pset_create does not grow with the number of views or points: one view's workspace
+ * (kept at the largest view added so far), plus the masks and one chunk of points during clipping.  A handle made by
+ * b200mvs_pset_create_on_device keeps its point set in DEVICE memory instead (below).  Errors: negative code,
+ * b200mvs_depthmap_last_error(). */
 typedef struct b200mvs_pset b200mvs_pset;
 typedef struct b200mvs_pset_options {
     int32_t with_normals;         /* -n: angle-weighted vertex normals                                              */
@@ -399,11 +401,12 @@ typedef struct b200mvs_pset_info {
     uint64_t n_points;            /* points in the set                                                              */
     uint64_t n_colors;            /* colours in the set: less than n_points when a view had no colour image          */
     uint64_t n_views;             /* views added (not skipped)                                                      */
-    uint64_t device_bytes;        /* device bytes the handle holds now                                              */
+    uint64_t device_bytes;        /* device bytes the handle holds now (a device-resident set's arrays included)     */
     uint64_t peak_device_bytes;   /* maximum of device_bytes since creation                                         */
     double   ms_pointset;         /* device time of the per-view kernels (triangulation, normals, confidences, scales) */
     double   ms_filter;           /* device time of fill count, bounding box, compaction, normal scaling, pixel map  */
-    double   ms_mask;             /* device time of mask clipping, including the transfers of the chunks              */
+    double   ms_mask;             /* device time of mask clipping: with the transfers of the chunks on a host-resident
+                                     set; clip, scan and compaction in place (no transfers) on a device-resident one */
 } b200mvs_pset_info;
 /* Correspondence metadata of one added view (scene2pset.cc:50-56). */
 typedef struct b200mvs_pset_corr_view {
@@ -412,6 +415,19 @@ typedef struct b200mvs_pset_corr_view {
 } b200mvs_pset_corr_view;
 
 int b200mvs_pset_create(int device, const b200mvs_pset_options* options, b200mvs_pset** out);
+/* A handle whose point set is kept in DEVICE memory on `device`; options are checked as b200mvs_pset_create checks them
+ * (the same codes and messages, naming this function).  Every b200mvs_pset_* entry point takes it with the same meaning
+ * and gives the same arrays, records and counts as for a b200mvs_pset_create handle fed the same inputs:
+ *   - views append their points with device-to-device copies; b200mvs_pset_add_reconstruction stages each view on the
+ *     device and commits them in ref_views order when the whole call succeeds (on an error, or every view cancelled,
+ *     the set is unchanged; its capacity may have grown);
+ *   - b200mvs_pset_clip_masks clips and compacts the set in place (the masks are uploaded once);
+ *   - b200mvs_pset_read / _read_correspondence copy the set to the host; b200mvs_pset_read_device copies it to device
+ *     buffers without a host copy.
+ * The set is the caller's memory, like the buffers of b200mvs_reconstruct_device: its arrays grow by doubling through
+ * cudaMalloc, are never taken from a context's budget (b200mvs_memory is the same for either kind of handle), and are
+ * counted in the handle's device_bytes and peak_device_bytes. */
+int b200mvs_pset_create_on_device(int device, const b200mvs_pset_options* options, b200mvs_pset** out);
 void b200mvs_pset_destroy(b200mvs_pset* ps);
 /* One view (scene2pset.cc:284-399): depth map w x h, colour image of the same size with 1-4 channels or NULL, camera.
  * The view's calibration for the map's size and its camera-to-world matrix are formed as CameraInfo forms them. */
@@ -437,6 +453,14 @@ int b200mvs_pset_get_info(b200mvs_pset* ps, b200mvs_pset_info* out);
 int b200mvs_pset_read(b200mvs_pset* ps, float* vertices, float* normals, float* colors, float* values, float* confidences);
 /* With options.correspondence: pixel (x, y) of every point, and one record per added view (n_views of them). */
 int b200mvs_pset_read_correspondence(b200mvs_pset* ps, uint32_t* pixels_xy, b200mvs_pset_corr_view* views);
+/* b200mvs_pset_read and the pixel map of b200mvs_pset_read_correspondence into DEVICE buffers on the handle's device, in
+ * the same layouts; NULL skips an array, and pixels_xy must be NULL on a handle made without correspondence.  Works on
+ * either kind of handle (a host-resident set is copied host to device).  Buffers are checked as b200mvs_reconstruct_device
+ * checks its maps (host memory, another device or a pointer not 4-byte aligned: B200MVS_ERR_INVALID_ARG naming the
+ * field) before anything is copied; the copies wait for an event recorded on cuda_stream (NULL = the legacy default
+ * stream) at entry, and the call returns when they are done. */
+int b200mvs_pset_read_device(b200mvs_pset* ps, float* vertices_dev, float* normals_dev, float* colors_dev, float* values_dev,
+                             float* confidences_dev, uint32_t* pixels_xy_dev, void* cuda_stream);
 
 /* ---- dmrecon straight into scene2pset: the point sets of a batch of reference views without their maps leaving the device ----
  * Bit-identical to b200mvs_reconstruct(ctx, s, n_refs, ref_views, maps, progress, stats, failed_view_or_null) followed, for

@@ -2778,8 +2778,8 @@ int b200mvs_pset_add_reconstruction(b200mvs_pset* ps, b200mvs_ctx* ctx, const b2
     PD::use_allocator(ps, &A);
     const int rc = reconstruct(ctx, s, n_refs, refs, nullptr, &sink, progress, stats, failed_view);
     PD::use_allocator(ps, nullptr);
-    if (rc) return rc;
-    PD::commit(ps, blocks, views_out);
+    if (rc) { PD::discard(ps); return rc; }
+    if (int crc = PD::commit(ps, blocks, views_out)) return fail(crc, "%s", b200mvs_depthmap_last_error());
     return 0;
 }
 

@@ -140,6 +140,8 @@ def _pset_lib():
     L = _lib()
     if not getattr(L, "_pset_ready", False):
         L.b200mvs_pset_create.argtypes = [C.c_int, C.POINTER(_PsetOptions), C.POINTER(C.c_void_p)]
+        L.b200mvs_pset_create_on_device.argtypes = [C.c_int, C.POINTER(_PsetOptions), C.POINTER(C.c_void_p)]
+        L.b200mvs_pset_read_device.argtypes = [C.c_void_p] + [C.c_void_p] * 7
         L.b200mvs_pset_destroy.argtypes = [C.c_void_p]
         L.b200mvs_pset_destroy.restype = None
         L.b200mvs_pset_add_view.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.POINTER(_PsetCamera),
@@ -186,8 +188,9 @@ def _view_record(view_id, r):
                 first_index=int(r.first_index))
 
 
-def _finish(L, h, o, masks, per_view):
-    """Clips the handle's points with `masks` and reads the point set out (the result of scene_pointset)."""
+def _finish(L, h, o, masks, per_view, device=None):
+    """Clips the handle's points with `masks` and reads the point set out (the result of scene_pointset): numpy arrays, or
+    with `device` (a handle's device index) torch CUDA tensors on that device, read on its current stream."""
     num_filtered = 0
     if masks:
         ms = [np.ascontiguousarray(m["mask"], np.uint8) for m in masks]
@@ -203,17 +206,29 @@ def _finish(L, h, o, masks, per_view):
     info = _PsetInfo()
     _check(L.b200mvs_pset_get_info(h, C.byref(info)))
     n, nc = int(info.n_points), int(info.n_colors)
-    verts = np.empty((n, 3), np.float32)
-    nrm = np.empty((n, 3), np.float32) if o["with_normals"] else None
-    cols = np.empty((nc, 4), np.float32)
-    vals = np.empty(n, np.float32) if o["with_scale"] else None
-    cfs = np.empty(n, np.float32) if o["with_conf"] else None
-    _check(L.b200mvs_pset_read(h, _p(verts), _p(nrm), _p(cols), _p(vals), _p(cfs)))
+    if device is None:
+        empty, f32, u32, ptr = np.empty, np.float32, np.uint32, _p
+    else:
+        import torch
+        dev = torch.device("cuda", device)
+        # uint32 where torch has the dtype (it copies and converts to numpy; few kernels take it), else the same bits as int32
+        empty, f32, u32 = (lambda shape, dt: torch.empty(shape, dtype=dt, device=dev)), torch.float32, getattr(torch, "uint32", torch.int32)
+        ptr = lambda t: None if t is None else C.c_void_p(t.data_ptr())             # noqa: E731
+    verts = empty((n, 3), f32)
+    nrm = empty((n, 3), f32) if o["with_normals"] else None
+    cols = empty((nc, 4), f32)
+    vals = empty(n, f32) if o["with_scale"] else None
+    cfs = empty(n, f32) if o["with_conf"] else None
+    pix = empty((n, 2), u32) if o["correspondence"] else None
+    if device is None:
+        _check(L.b200mvs_pset_read(h, _p(verts), _p(nrm), _p(cols), _p(vals), _p(cfs)))
+    else:
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        _check(L.b200mvs_pset_read_device(h, ptr(verts), ptr(nrm), ptr(cols), ptr(vals), ptr(cfs), ptr(pix), C.c_void_p(stream)))
     corr = None
     if o["correspondence"]:
-        pix = np.empty((n, 2), np.uint32)
         meta = (_PsetCorrView * max(1, int(info.n_views)))()
-        _check(L.b200mvs_pset_read_correspondence(h, _p(pix), meta))
+        _check(L.b200mvs_pset_read_correspondence(h, _p(pix) if device is None else None, meta))
         corr = dict(pixels=pix, views=[(int(m.view_id), int(m.width), int(m.height), int(m.first_index))
                                        for m in meta[:int(info.n_views)]])
     return dict(vertices=verts, normals=nrm, colors=cols, values=vals, confidences=cfs, views=per_view, correspondence=corr,
@@ -222,7 +237,14 @@ def _finish(L, h, o, masks, per_view):
                           ms_pointset=info.ms_pointset, ms_filter=info.ms_filter, ms_mask=info.ms_mask))
 
 
-def scene_pointset(views, options=None, masks=None, device: int = 0):
+def _create(L, device, opt, on_device):
+    h = C.c_void_p()
+    create = L.b200mvs_pset_create_on_device if on_device else L.b200mvs_pset_create
+    _check(create(device, C.byref(opt), C.byref(h)))
+    return h
+
+
+def scene_pointset(views, options=None, masks=None, device: int = 0, on_device: bool = False):
     """The whole-scene point set of apps/scene2pset (scene2pset.cc:247-464) on the device, through b200mvs_pset_*.
 
     views: dicts with id, depth [H, W] float32, camera (dict of flen, paspect, ppoint, rot, trans as in mve::CameraInfo) and
@@ -236,11 +258,15 @@ def scene_pointset(views, options=None, masks=None, device: int = 0):
     Returns dict(vertices [N, 3], normals [N, 3] or None, colors [M, 4] (M < N when a view had no colour image),
     values [N] or None, confidences [N] or None, views (per input view: id, added, fraction, n_points, first_index),
     correspondence (pixels [N, 2] uint32, views [(view_id, width, height, first_index)]) or None, num_filtered,
-    info (peak_device_bytes, device_bytes, ms_pointset, ms_filter, ms_mask))."""
+    info (peak_device_bytes, device_bytes, ms_pointset, ms_filter, ms_mask)).
+
+    on_device: the set is built and clipped in device memory (b200mvs_pset_create_on_device) and vertices, normals,
+    colors, values, confidences and correspondence pixels are torch CUDA tensors on `device`, read on its current stream
+    (b200mvs_pset_read_device), with the shapes and dtypes above; the pixels are torch.uint32 (torch.int32 with the same
+    bits on a torch without uint32).  views, correspondence views, num_filtered and info stay host values."""
     o, opt = _options(options)
     L = _pset_lib()
-    h = C.c_void_p()
-    _check(L.b200mvs_pset_create(device, C.byref(opt), C.byref(h)))
+    h = _create(L, device, opt, on_device)
     try:
         per_view = []
         for v in views:
@@ -259,7 +285,7 @@ def scene_pointset(views, options=None, masks=None, device: int = 0):
             cam = _camera(v["camera"])
             _check(L.b200mvs_pset_add_view(h, int(v["id"]), _p(dm), dm.shape[1], dm.shape[0], _p(col), cch, C.byref(cam), C.byref(r)))
             per_view.append(_view_record(v["id"], r))
-        return _finish(L, h, o, masks, per_view)
+        return _finish(L, h, o, masks, per_view, device if on_device else None)
     finally:
         L.b200mvs_pset_destroy(h)
 
@@ -292,19 +318,20 @@ def _add_device_view(L, h, v):
     return _view_record(v["id"], r)
 
 
-def reconstruct_pointset(scene, settings, ref_views, options=None, masks=None, progress=None):
+def reconstruct_pointset(scene, settings, ref_views, options=None, masks=None, progress=None, on_device: bool = False):
     """dmrecon and scene2pset in one call (b200mvs_pset_add_reconstruction): reconstructs the reference views of
     `scene` (a dmrecon.Scene) and builds their point set on the device, each view's depth map and colours (its pyramid
     level settings.scale) staying on the device.  Equal to scene.reconstruct(...) followed by scene_pointset of the maps
-    with the level images and the registered cameras, in ref_views order.  options and masks as for scene_pointset;
-    progress as for Scene.reconstruct.  Returns (the dict of scene_pointset, dmrecon.Stats)."""
+    with the level images and the registered cameras, in ref_views order.  options, masks and on_device as for
+    scene_pointset (on_device: the set never leaves the scene's device); progress as for Scene.reconstruct.  Returns
+    (the dict of scene_pointset, dmrecon.Stats)."""
     o, opt = _options(options)
     L = _pset_lib()
     refs = np.asarray(ref_views, np.int32)
     h = C.c_void_p()
     # a planning context has no device to make a handle on: the call itself rejects the context
     if scene.device != dmrecon.DEVICE_NONE:
-        _check(L.b200mvs_pset_create(scene.device, C.byref(opt), C.byref(h)))
+        h = _create(L, scene.device, opt, on_device)
     try:
         recs = (_PsetView * max(1, len(refs)))()
         stats = dmrecon.Stats()
@@ -317,7 +344,7 @@ def reconstruct_pointset(scene, settings, ref_views, options=None, masks=None, p
                 msg += " (view %d)" % failed.value
             raise dmrecon.B200MVSError(rc, msg, failed.value)
         per_view = [_view_record(v, recs[j]) for j, v in enumerate(refs.tolist())]
-        return _finish(L, h, o, masks, per_view), stats
+        return _finish(L, h, o, masks, per_view, scene.device if on_device else None), stats
     finally:
         if h.value:
             L.b200mvs_pset_destroy(h)

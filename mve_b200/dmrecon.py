@@ -85,7 +85,7 @@ EXPORTS = ["b200mvs_default_settings", "b200mvs_create", "b200mvs_destroy", "b20
            "b200mvs_set_frontier_capacity", "b200mvs_frontier_info", "b200mvs_plan_stats", "b200mvs_pset_create", "b200mvs_pset_destroy",
            "b200mvs_pset_add_view", "b200mvs_pset_clip_masks", "b200mvs_pset_get_info", "b200mvs_pset_read",
            "b200mvs_pset_read_correspondence", "b200mvs_pset_add_reconstruction", "b200mvs_reconstruct_device",
-           "b200mvs_get_level_device", "b200mvs_pset_add_view_device"]
+           "b200mvs_get_level_device", "b200mvs_pset_add_view_device", "b200mvs_pset_create_on_device", "b200mvs_pset_read_device"]
 
 ERR_INVALID_ARG = -1
 ERR_CUDA = -2
@@ -485,12 +485,14 @@ class Scene:
         self._raise(rc, failed)
         return results, stats
 
-    def reconstruct_pointset(self, settings: Settings, ref_views: Sequence[int], options=None, masks=None, progress=None):
+    def reconstruct_pointset(self, settings: Settings, ref_views: Sequence[int], options=None, masks=None, progress=None,
+                             on_device: bool = False):
         """DMRecon::start for a batch of reference views and scene2pset of their maps, without the maps leaving the device
-        (b200mvs_pset_add_reconstruction).  options / masks: as for mve_b200.depthmap.scene_pointset (the masks are applied
-        after the reconstruction); progress: as for reconstruct().  Returns (the dict of depthmap.scene_pointset, Stats)."""
+        (b200mvs_pset_add_reconstruction).  options / masks / on_device: as for mve_b200.depthmap.scene_pointset (the masks
+        are applied after the reconstruction; on_device keeps the point set on the device and returns CUDA tensors);
+        progress: as for reconstruct().  Returns (the dict of depthmap.scene_pointset, Stats)."""
         from . import depthmap
-        return depthmap.reconstruct_pointset(self, settings, ref_views, options, masks, progress)
+        return depthmap.reconstruct_pointset(self, settings, ref_views, options, masks, progress, on_device)
 
 
 class DMRecon:
