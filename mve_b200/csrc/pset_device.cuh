@@ -1,7 +1,7 @@
 // The point-set handle's side of b200mvs_pset_add_reconstruction.  b200mvs.cu runs the reconstruction and hands every
 // finished depth map, still on the device, to the handle of depthmap.cu together with the view's pyramid level and camera;
-// each view's points are held per view (on the host, or staged on the device for a device-resident set) and committed in
-// the caller's view order when the whole call succeeded.
+// each view's points are staged behind the handle's set and committed in the caller's view order when the whole call
+// succeeded.
 #pragma once
 #include "../../include/b200mvs.h"
 
@@ -12,28 +12,22 @@
 
 namespace b200mvs_pset_dev {
 
-// A point list of the handle, or the points of one view before they are committed
-struct Points {
-    std::vector<float> verts, normals, colors, values, confs;
-    std::vector<uint32_t> pix;                                   // correspondence: (x, y) per point
-};
-
-// The point set of a handle made by b200mvs_pset_create_on_device: the lists of Points in device memory, 4-byte items,
-// PER[k] of them per entry.  List k holds n[k] committed entries followed by staged[k] entries that a view appended and
-// that are not part of the set until they are committed; cap[k] entries fit.
-struct DevPoints {
+// The point set of a handle: lists of 4-byte items, PER[k] of them per entry (PIX: the (x, y) of each point for the
+// correspondence).  They live in device memory for a handle made by b200mvs_pset_create_on_device and in host memory
+// otherwise.  List k holds n[k] committed entries followed by staged[k] entries that a view appended and that are not part
+// of the set until they are committed; cap[k] entries fit.
+struct Lists {
     enum { VERTS, NORMALS, COLORS, VALUES, CONFS, PIX, N_LISTS };
     static constexpr int PER[N_LISTS] = {3, 3, 4, 1, 1, 2};
+    bool on_device = false;
     void* p[N_LISTS] = {};
     uint64_t n[N_LISTS] = {}, staged[N_LISTS] = {}, cap[N_LISTS] = {};
 };
 
-// The points of one reference view, held until the call commits them: in `pts` for a host-resident set, at
-// [at[k], at[k] + count[k]) of the staged entries of list k for a device-resident one
+// The points of one reference view until the call commits them: [at[k], at[k] + count[k]) of list k, staged
 struct Block {
     b200mvs_pset_view rec = {0, 0.f, 0, 0};          // first_index is set by commit
-    Points pts;
-    uint64_t at[DevPoints::N_LISTS] = {}, count[DevPoints::N_LISTS] = {};
+    uint64_t at[Lists::N_LISTS] = {}, count[Lists::N_LISTS] = {};
     uint32_t view_id = 0, width = 0, height = 0;
     double ms_pointset = 0, ms_filter = 0;
 };
@@ -53,11 +47,11 @@ uint64_t workspace_bytes(const b200mvs_pset* ps, int w, int h);
 // Frees the workspace, then allocates it through `a` from here on (NULL: cudaMalloc)
 void use_allocator(b200mvs_pset* ps, const Allocator* a);
 // What b200mvs_pset_add_view does with the map and a 3-channel colour image, for a DEVICE depth map (w x h floats) and
-// colours read in place from an RGBX level (uchar4, row pitch `pitch` texels); the points go to `out`, not to the handle
+// colours read in place from an RGBX level (uchar4, row pitch `pitch` texels); the points are staged, `out` records where
 int extract(b200mvs_pset* ps, int view_id, const float* d_depth, int w, int h, const void* d_rgbx, int pitch,
             const b200mvs_pset_camera& cam, Block& out);
-// Appends the blocks to the handle in their order; records[j] receives block j's record (records may be NULL).  On an
-// error (a device-resident set that could not put its staged points in order) the set is as before the call.
+// Commits the staged blocks to the handle in their order; records[j] receives block j's record (records may be NULL).  On
+// an error (the staged points could not be put in order) the set is as before the call.
 int commit(b200mvs_pset* ps, const std::vector<Block>& blocks, b200mvs_pset_view* records);
 // Forgets what extract staged since the last commit (a call that failed): the set is as before the call
 void discard(b200mvs_pset* ps);
