@@ -165,6 +165,18 @@ int b200mvs_upload_view_device(b200mvs_ctx* ctx, int view_id, const uint8_t* rgb
  * needed image is missing. */
 int b200mvs_set_view_camera(b200mvs_ctx* ctx, int view_id, int w, int h, float flen, float paspect,
                             const float ppoint[2], const float rot[9], const float trans[3]);
+/* Radial distortion of the images this view is given, as sfmrecon undistorts a view's `original` photo into its
+ * `undistorted` image (apps/sfmrecon/sfmrecon.cc:425-437): k2, k4 are CameraInfo::dist[0], dist[1] (camera.h:161-162,
+ * meta.ini camera.radial_distortion).  Every later b200mvs_upload_view, b200mvs_upload_view_device and image-source fetch
+ * of the view then takes the distorted photo, and level 0 of its pyramid is byte for byte
+ * mve::image::image_undistort_k2k4<uint8_t>(photo, flen, k2, k4) (image_tools.h:1731-1769) with the flen the view is
+ * registered with.  k2 == k4 == 0 (the default) imports the image unchanged, as the reference's duplicate() does.
+ * Changing the values drops a resident pyramid: with an image source the view is fetched again when a call needs it;
+ * without one a reconstruction fails with "color image of view N is not loaded" until the view is uploaded again.
+ * Cameras and prepared plans are untouched (the geometry stays pinhole, as for the `undistorted` image), no memory is
+ * allocated, and it works in a planning context, where it only stores the values.  Non-finite values or a bad view id:
+ * B200MVS_ERR_INVALID_ARG. */
+int b200mvs_set_view_distortion(b200mvs_ctx* ctx, int view_id, float k2, float k4);
 /* mve::Bundle::Features (bundle.h:51-60) as position + CSR list of referencing view ids. */
 int b200mvs_set_features(b200mvs_ctx* ctx, int n_features, const float* pos,
                          const int32_t* ref_offsets, const int32_t* ref_view_ids);

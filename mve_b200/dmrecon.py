@@ -85,7 +85,8 @@ EXPORTS = ["b200mvs_default_settings", "b200mvs_create", "b200mvs_destroy", "b20
            "b200mvs_set_frontier_capacity", "b200mvs_frontier_info", "b200mvs_plan_stats", "b200mvs_pset_create", "b200mvs_pset_destroy",
            "b200mvs_pset_add_view", "b200mvs_pset_clip_masks", "b200mvs_pset_get_info", "b200mvs_pset_read",
            "b200mvs_pset_read_correspondence", "b200mvs_pset_add_reconstruction", "b200mvs_reconstruct_device",
-           "b200mvs_get_level_device", "b200mvs_pset_add_view_device", "b200mvs_pset_create_on_device", "b200mvs_pset_read_device"]
+           "b200mvs_get_level_device", "b200mvs_pset_add_view_device", "b200mvs_pset_create_on_device", "b200mvs_pset_read_device",
+           "b200mvs_set_view_distortion"]
 
 ERR_INVALID_ARG = -1
 ERR_CUDA = -2
@@ -142,6 +143,7 @@ def lib():
     L.b200mvs_upload_view_device.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float,
                                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.b200mvs_set_features.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.b200mvs_set_view_distortion.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_float]
     L.b200mvs_set_view_camera.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
     L.b200mvs_num_levels.argtypes = [C.c_void_p, C.c_int]
     L.b200mvs_get_level.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -300,6 +302,13 @@ class Scene:
         r = np.ascontiguousarray(rot, np.float32).reshape(9)
         t = np.ascontiguousarray(trans, np.float32).reshape(3)
         self._check(self._lib.b200mvs_set_view_camera(self._h, view_id, w, h, float(flen), float(paspect), _p(pp), _p(r), _p(t)))
+
+    def set_view_distortion(self, view_id: int, k2: float, k4: float):
+        """Radial distortion (mve::CameraInfo::dist, meta.ini camera.radial_distortion) of the images this view is given
+        from now on: set_view, set_view_device and image-source fetches take the distorted photo, and level(view, 0) is
+        sfmrecon's undistortion of it (mve::image::image_undistort_k2k4 with the view's flen).  (0, 0), the default,
+        imports images unchanged.  A changed value drops the view's resident pyramid; cameras are unchanged."""
+        self._check(self._lib.b200mvs_set_view_distortion(self._h, view_id, float(k2), float(k4)))
 
     def set_features(self, pos: np.ndarray, refs: Sequence[np.ndarray]):
         """mve::Bundle::Features (bundle.h:51-60)."""

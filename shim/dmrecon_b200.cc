@@ -149,6 +149,14 @@ void release_image(void* user, int32_t id)
     D.scene->get_views()[id]->cache_cleanup();
 }
 
+// B200MVS_UNDISTORT=1: the images read (-i, default `undistorted`) are distorted photos, undistorted on the device with each
+// view's camera.radial_distortion (b200mvs_set_view_distortion); unset or 0, they are used as they are.
+bool undistort_images()
+{
+    const char* e = std::getenv("B200MVS_UNDISTORT");
+    return e != nullptr && std::strcmp(e, "0") != 0 && *e != '\0';
+}
+
 // Device budget of a context: B200MVS_DEVICE_BUDGET_MB, or 0 = 90 % of the free device memory (include/b200mvs.h).
 uint64_t device_budget()
 {
@@ -322,6 +330,10 @@ DMRecon::start()
             mve::CameraInfo const& cam = v->get_camera();
             int rc = b200mvs_set_view_camera(ctx, (int)i, proxy->width, proxy->height, cam.flen, cam.paspect, cam.ppoint,
                 cam.rot, cam.trans);
+            /* B200MVS_UNDISTORT=1: the embedding holds the distorted photo; undistort it with the view's
+               camera.radial_distortion as sfmrecon does (sfmrecon.cc:425-437) */
+            if (rc == 0 && undistort_images())
+                rc = b200mvs_set_view_distortion(ctx, (int)i, cam.dist[0], cam.dist[1]);
             if (rc != 0) throw_for(rc, b200mvs_last_error(ctx));
         }
         D.cameras_set = true;
