@@ -316,6 +316,44 @@ typedef void (*b200mvs_release_fn)(void* user, int32_t view_id);
 int b200mvs_set_image_source(b200mvs_ctx* ctx, b200mvs_fetch_fn fetch, b200mvs_release_fn release, void* user,
                              uint64_t budget_bytes);
 
+/* An image source whose images are in DEVICE memory, e.g. decoded on the GPU or held as CUDA tensors.  Texel (x, y),
+ * channel c lies at data + y * row_pitch + x * channels + c when plane_pitch == 0 (interleaved, HWC) and at
+ * data + c * plane_pitch + y * row_pitch + x when plane_pitch > 0 (planar, CHW). */
+typedef struct b200mvs_device_image {
+    const uint8_t* data;          /* DEVICE pointer on the context's device; valid until the release callback             */
+    int32_t w, h, channels;       /* must equal the registered size; channels 1..4 (grey expanded, alpha dropped)        */
+    int64_t row_pitch;            /* bytes between rows; >= w * channels interleaved, >= w planar                        */
+    int64_t plane_pitch;          /* 0 = interleaved (HWC); else planar (CHW): bytes between channel planes, >= h * row_pitch */
+    void*   cuda_stream;          /* cudaStream_t the image was produced on (NULL = the legacy default stream)             */
+} b200mvs_device_image;
+/* Returns 0 and fills *out with the `undistorted` image of view_id (or the distorted photo, b200mvs_set_view_distortion),
+ * non-zero when it cannot be loaded. */
+typedef int (*b200mvs_device_fetch_fn)(void* user, int32_t view_id, b200mvs_device_image* out);
+/* Installs (fetch != NULL) or removes (fetch == NULL) a device image source.  A context has one source: installing either
+ * kind replaces the other, and removing either removes it.
+ *   - As b200mvs_set_image_source: the budget and budget_bytes = 0, which calls fetch and when, LRU eviction, the groups
+ *     of b200mvs_reconstruct, the context lock held during the callbacks, and the failure messages and failed_view of a
+ *     fetch that fails.
+ *   - Accounting: b200mvs_memory is kept as for a host source, so both plan the same groups, evict the same pyramids and
+ *     report the same numbers over the same scene.  The pyramid is built straight from the caller's memory, with no
+ *     staging copy; the budget is still charged the two staging buffers a host source would allocate (fixed keeps their
+ *     bound).  n_loads counts the device fetches and bytes_loaded their w * h * channels.  The caller's image memory is
+ *     not in the budget.
+ *   - Ordering: when fetch returns, the library records an event on cuda_stream and its kernels wait for it before they
+ *     read the image, so fetch may enqueue the decode and return without synchronising.
+ *   - Release: release (may be NULL) is called once per successful fetch, after every kernel that reads the image has
+ *     completed and before the call that fetched it returns.  The library waits for those kernels once per batch of
+ *     loads (one b200mvs_reconstruct group, one b200mvs_get_level, ...), never with cudaDeviceSynchronize.
+ *   - Before anything reads the image, the descriptor is checked: data must be device (or managed) memory on the
+ *     context's device (cudaPointerGetAttributes, as for the maps of b200mvs_reconstruct_device: host memory, pinned or
+ *     pageable, and memory of another device are rejected), w and h the registered size, channels 1..4, row_pitch and
+ *     plane_pitch non-negative and within the bounds above (a plane_pitch below h * row_pitch would overlap the rows of
+ *     a plane).  A failed check gives B200MVS_ERR_INVALID_ARG with a message naming the view (failed_view as for a
+ *     failed fetch); release is still called, nothing is launched, and the context stays usable.  The caller keeps the
+ *     whole extent of the image within one allocation. */
+int b200mvs_set_image_source_device(b200mvs_ctx* ctx, b200mvs_device_fetch_fn fetch, b200mvs_release_fn release, void* user,
+                                    uint64_t budget_bytes);
+
 typedef struct b200mvs_memory {
     uint64_t budget;              /* 0 = no source installed (no limit)                                           */
     uint64_t fixed;               /* bytes that do not depend on the batch: view table, sRGB table, settings and frontier

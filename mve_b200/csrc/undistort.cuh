@@ -1,6 +1,7 @@
 // sfmrecon's radial undistortion of a view's `original` photo (sfmrecon.cc:425-437): mve::image::image_undistort_k2k4<uint8_t>
 // (image_tools.h:1731-1769) with Image::linear_at(float, float, T*) (image.h:438-460) and the four-value unsigned char
 // math::interpolate (functions.h:141-147), one output pixel per call, bit for bit as the reference build computes it.
+// The source may be packed or pitched HWC, or planar CHW (Src): only where a texel is read from depends on the layout.
 // That build (-O3 -march=x86-64-v3 -funsafe-math-optimizations) does not evaluate the source as written; its instantiation
 // (tests/undistort_reference.py restates it) does, per image:
 //     fwidth2 = w * 0.5, fheight2 = h * 0.5, inv_fnorm = 1 / max(w, h), inv_f2 = 1 / (flen * flen)       (double)
@@ -62,6 +63,20 @@ struct Params {
     int w, h, ch;           // image size and channels (1..4)
 };
 
+// Where the source image lies: texel (x, y), channel c at base + y * row + x * ch + c when interleaved (HWC; packed when
+// row = w * ch), at base + c * plane + y * row + x when planar (CHW).  The layout is a template parameter of the readers,
+// so the packed path computes its addresses as before and no texel read branches on it.
+struct Src {
+    const uint8_t* base;
+    int64_t row;            // bytes between rows
+    int64_t plane;          // bytes between channel planes (planar only)
+};
+template <bool Planar> UNDIST_FN const uint8_t* texel(const Src& s, int ch, int x, int y)
+{
+    return s.base + (int64_t)y * s.row + (int64_t)x * (Planar ? 1 : ch);
+}
+template <bool Planar> UNDIST_FN int64_t channel_offset(const Src& s, int c) { return Planar ? c * s.plane : c; }
+
 // k2 == k4 == 0 is the reference's duplicate(): the caller imports the image unchanged instead
 inline bool active(float k2, float k4) { return k2 != 0.0f || k4 != 0.0f; }
 
@@ -84,8 +99,8 @@ inline Params make_params(int w, int h, int ch, float flen, float k2, float k4)
 }
 
 // The channels of output pixel (x, y) of image_undistort_k2k4, channel c in bits 8c..8c+7 (0 where the reference leaves
-// the pixel 0, and above channel ch - 1); src is the h x w x ch source image, row-major
-UNDIST_FN uint32_t undistort_px(const Params& P, const uint8_t* src, int x, int y)
+// the pixel 0, and above channel ch - 1), read from the w x h x ch source image `src`
+template <bool Planar> UNDIST_FN uint32_t undistort_px(const Params& P, const Src& src, int x, int y)
 {
     const double fx = dmul(dadd((double)x, P.ox), P.inv_fnorm);
     const double fy = dmul(dadd((double)y, P.oy), P.inv_fnorm);
@@ -105,20 +120,26 @@ UNDIST_FN uint32_t undistort_px(const Params& P, const uint8_t* src, int x, int 
     const int y1 = y0 + 1 < P.h - 1 ? y0 + 1 : P.h - 1;
     const float w1 = fsub(ix, tx), w0 = fadd(tx, fsub(1.0f, ix));
     const float w3 = fsub(iy, ty), w2 = fsub(fadd(ty, 1.0f), iy);
-    const size_t row0 = (size_t)y0 * P.w, row1 = (size_t)y1 * P.w;
-    const uint8_t* p00 = src + (row0 + x0) * P.ch;
-    const uint8_t* p01 = src + (row0 + x1) * P.ch;
-    const uint8_t* p10 = src + (row1 + x0) * P.ch;
-    const uint8_t* p11 = src + (row1 + x1) * P.ch;
+    const uint8_t* p00 = texel<Planar>(src, P.ch, x0, y0);
+    const uint8_t* p01 = texel<Planar>(src, P.ch, x1, y0);
+    const uint8_t* p10 = texel<Planar>(src, P.ch, x0, y1);
+    const uint8_t* p11 = texel<Planar>(src, P.ch, x1, y1);
     uint32_t out = 0u;
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
         if (c >= P.ch) break;
-        const float top = ffma((float)load_u8(p00 + c), w0, fmul((float)load_u8(p01 + c), w1));
-        const float bot = ffma((float)load_u8(p10 + c), w0, fmul((float)load_u8(p11 + c), w1));
+        const int64_t o = channel_offset<Planar>(src, c);
+        const float top = ffma((float)load_u8(p00 + o), w0, fmul((float)load_u8(p01 + o), w1));
+        const float bot = ffma((float)load_u8(p10 + o), w0, fmul((float)load_u8(p11 + o), w1));
         out |= (uint32_t)(f2i_rz(fadd(ffma(top, w2, fmul(bot, w3)), 0.5f)) & 0xFF) << (8 * c);
     }
     return out;
+}
+
+// The same from a packed h x w x ch image
+UNDIST_FN uint32_t undistort_px(const Params& P, const uint8_t* src, int x, int y)
+{
+    return undistort_px<false>(P, Src{src, (int64_t)P.w * P.ch, 0}, x, y);
 }
 
 } // namespace b200mvs_undistort

@@ -86,7 +86,7 @@ EXPORTS = ["b200mvs_default_settings", "b200mvs_create", "b200mvs_destroy", "b20
            "b200mvs_pset_add_view", "b200mvs_pset_clip_masks", "b200mvs_pset_get_info", "b200mvs_pset_read",
            "b200mvs_pset_read_correspondence", "b200mvs_pset_add_reconstruction", "b200mvs_reconstruct_device",
            "b200mvs_get_level_device", "b200mvs_pset_add_view_device", "b200mvs_pset_create_on_device", "b200mvs_pset_read_device",
-           "b200mvs_set_view_distortion"]
+           "b200mvs_set_view_distortion", "b200mvs_set_image_source_device"]
 
 ERR_INVALID_ARG = -1
 ERR_CUDA = -2
@@ -101,8 +101,63 @@ class _Image(C.Structure):
     _fields_ = [("rgb", C.c_void_p), ("w", C.c_int32), ("h", C.c_int32), ("channels", C.c_int32)]
 
 
+class _DeviceImage(C.Structure):
+    """b200mvs_device_image (include/b200mvs.h)."""
+    _fields_ = [("data", C.c_void_p), ("w", C.c_int32), ("h", C.c_int32), ("channels", C.c_int32),
+                ("row_pitch", C.c_int64), ("plane_pitch", C.c_int64), ("cuda_stream", C.c_void_p)]
+
+
 _FETCH_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int32, C.POINTER(_Image))
+_DEVICE_FETCH_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int32, C.POINTER(_DeviceImage))
 _RELEASE_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_int32)
+
+
+def device_image_layout(shape: Sequence[int], strides: Sequence[int], layout: str = "hwc"):
+    """The b200mvs_device_image fields (h, w, channels, row_pitch, plane_pitch) of a uint8 image of this shape and these
+    strides (in elements = bytes): layout "hwc" takes H x W x C or H x W (grey), "chw" takes C x H x W.  The element
+    stride must be 1, the pixel stride C (hwc) or 1 (chw), the row stride at least the bytes of a row and the plane stride
+    at least h * row stride (planes that do not overlap the rows of another).  The stride of a dimension of size 1 is never
+    used and is not checked.  Anything else raises ValueError."""
+    shape, strides = tuple(int(v) for v in shape), tuple(int(v) for v in strides)
+    if layout == "hwc":
+        if len(shape) == 2:
+            shape, strides = shape + (1,), strides + (1,)
+        if len(shape) != 3:
+            raise ValueError("an hwc image is H x W x C or H x W, not %s" % (shape,))
+        h, w, c = shape
+        row, px, el = strides
+        plane = 0
+    elif layout == "chw":
+        if len(shape) != 3:
+            raise ValueError("a chw image is C x H x W, not %s" % (shape,))
+        c, h, w = shape
+        plane, row, px = strides
+        el = 1
+    else:
+        raise ValueError("layout must be 'hwc' or 'chw', not %r" % (layout,))
+    if not 1 <= c <= 4:
+        raise ValueError("an image has 1 to 4 channels, not %d" % c)
+    if h < 1 or w < 1:
+        raise ValueError("empty image %s" % (shape,))
+    if c == 1 and layout == "hwc":
+        el = 1
+    if layout == "hwc":
+        if el != 1 or (w > 1 and px != c):
+            raise ValueError("an hwc image needs channel stride 1 and pixel stride C, not strides %s" % (strides,))
+        row = row if h > 1 else w * c
+        if row < w * c:
+            raise ValueError("hwc row stride %d is less than W * C = %d" % (row, w * c))
+        return h, w, c, row, 0
+    if w > 1 and px != 1:
+        raise ValueError("a chw image needs pixel stride 1, not strides %s" % (strides,))
+    row = row if h > 1 else w
+    if row < w:
+        raise ValueError("chw row stride %d is less than W = %d" % (row, w))
+    plane = plane if c > 1 else h * row
+    if plane < h * row:
+        raise ValueError("chw plane stride %d overlaps the rows of a plane: it must be at least H * row stride = %d"
+                         % (plane, h * row))
+    return h, w, c, row, plane
 
 
 class Memory(C.Structure):
@@ -158,6 +213,7 @@ def lib():
     L.b200mvs_plan_views.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
     L.b200mvs_set_patch_mode.argtypes = [C.c_void_p, C.c_int, C.c_int64]
     L.b200mvs_set_image_source.argtypes = [C.c_void_p, _FETCH_FN, _RELEASE_FN, C.c_void_p, C.c_uint64]
+    L.b200mvs_set_image_source_device.argtypes = [C.c_void_p, _DEVICE_FETCH_FN, _RELEASE_FN, C.c_void_p, C.c_uint64]
     L.b200mvs_memory_stats.argtypes = [C.c_void_p, C.c_void_p]
     L.b200mvs_working_set.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
     L.b200mvs_plan_batches.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]
@@ -204,8 +260,18 @@ class Scene:
 
     def _check(self, rc: int):
         if rc < 0:
+            self._raise_fetch_error()
             raise B200MVSError(rc, self._lib.b200mvs_last_error(self._h).decode())
         return rc
+
+    def _raise_fetch_error(self):
+        """A device source's fetch returned a tensor that does not fit b200mvs_device_image: the failed call raises that
+        ValueError (the fetch itself could only return failure to the library)."""
+        errors = getattr(self, "_fetch_errors", None)
+        if errors:
+            err = errors[-1]
+            errors.clear()
+            raise err
 
     @classmethod
     def from_synth(cls, s, device: int = 0, views: Optional[Sequence[int]] = None, lazy: bool = False,
@@ -224,10 +290,18 @@ class Scene:
             sc.set_image_source(lambda v: s.images[v], budget_bytes)
         return sc
 
-    def set_image_source(self, fetch, budget_bytes: int = 0):
+    def set_image_source(self, fetch, budget_bytes: int = 0, on_device: bool = False, layout: str = "hwc"):
         """Loads images on demand: fetch(view_id) returns the view's H x W x C uint8 image (the size registered for the view).
         budget_bytes bounds the device memory of this context (0 = 90 % of the free bytes now); pyramids no running call
-        needs are evicted and fetched again when needed.  fetch=None removes the source."""
+        needs are evicted and fetched again when needed.  fetch=None removes the source.
+        on_device: fetch returns a torch.uint8 CUDA tensor on cuda:<device> instead (b200mvs_set_image_source_device):
+        H x W x C or H x W with layout "hwc", C x H x W with layout "chw", with any strides device_image_layout accepts.
+        The pyramid is built from the tensor in place, after the work enqueued on the current stream when fetch returns;
+        the tensor is held until the library releases it.  A tensor that does not fit makes the call that fetched it
+        raise ValueError."""
+        if on_device and fetch is not None:
+            self._set_device_source(fetch, budget_bytes, layout)
+            return
         held = {}
 
         def _fetch(_user, view_id, out):
@@ -252,6 +326,39 @@ class Scene:
         cbs = (_FETCH_FN(_fetch), _RELEASE_FN(_release), held)
         self._check(self._lib.b200mvs_set_image_source(self._h, cbs[0], cbs[1], None, int(budget_bytes)))
         self._source = cbs                       # the C side keeps the function pointers: keep the ctypes objects alive
+
+    def _set_device_source(self, fetch, budget_bytes: int, layout: str):
+        if layout not in ("hwc", "chw"):
+            raise ValueError("layout must be 'hwc' or 'chw', not %r" % (layout,))
+        torch = _torch()
+        dev = torch.device(self._torch_device())
+        held = {}
+        errors = []
+
+        def _fetch(_user, view_id, out):
+            try:
+                t = fetch(int(view_id))
+                if not isinstance(t, torch.Tensor) or t.dtype != torch.uint8 or t.device != dev:
+                    raise ValueError("fetch(%d) must return a torch.uint8 tensor on %s" % (view_id, dev))
+                h, w, c, row, plane = device_image_layout(t.shape, t.stride(), layout)
+                held[int(view_id)] = t
+                o = out.contents
+                o.data, o.w, o.h, o.channels, o.row_pitch, o.plane_pitch = t.data_ptr(), w, h, c, row, plane
+                o.cuda_stream = torch.cuda.current_stream(dev).cuda_stream
+                return 0
+            except ValueError as e:
+                errors.append(e)
+                return 1
+            except Exception:
+                return 1
+
+        def _release(_user, view_id):
+            held.pop(int(view_id), None)
+
+        cbs = (_DEVICE_FETCH_FN(_fetch), _RELEASE_FN(_release), held)
+        self._check(self._lib.b200mvs_set_image_source_device(self._h, cbs[0], cbs[1], None, int(budget_bytes)))
+        self._source = cbs                       # the C side keeps the function pointers: keep the ctypes objects alive
+        self._fetch_errors = errors
 
     def memory_stats(self) -> Memory:
         m = Memory()
@@ -447,6 +554,7 @@ class Scene:
 
     def _raise(self, rc: int, failed):
         if rc != 0:
+            self._raise_fetch_error()
             msg = self._lib.b200mvs_last_error(self._h).decode()
             if failed.value >= 0:
                 msg += " (view %d)" % failed.value
