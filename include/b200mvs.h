@@ -177,6 +177,20 @@ int b200mvs_set_view_camera(b200mvs_ctx* ctx, int view_id, int w, int h, float f
  * allocated, and it works in a planning context, where it only stores the values.  Non-finite values or a bad view id:
  * B200MVS_ERR_INVALID_ARG. */
 int b200mvs_set_view_distortion(b200mvs_ctx* ctx, int view_id, float k2, float k4);
+/* Reconstruction mask of a reference view: w x h bytes, row-major, 0 = background (the convention of scene2pset -m).
+ * When the view is reconstructed at level `scale` (maps W x H), its pixel (x, y) is background when mask pixel
+ * (floor((2x+1) w / 2W), floor((2y+1) h / 2H)) is 0, in integer arithmetic: a mask of the map's size maps one to one, a
+ * mask of the photo's size gives the photo pixel under the level pixel's centre.  A feature seed on a background pixel is
+ * dropped before the launch (it counts in neither n_seeds_processed nor n_seeds_success), no queue entry is ever made for
+ * a background pixel, and background pixels end as unfilled ones do: depth, conf, dz and normal 0, view ids -1; they are
+ * not counted in progress.filled or n_filled, and no point of b200mvs_pset_add_reconstruction comes from one.  Foreground
+ * pixels follow the unmasked rules.  b200mvs_reconstruct, b200mvs_reconstruct_device and b200mvs_pset_add_reconstruction
+ * apply it, with or without a budget.  Masks leave view selection, plans, b200mvs_working_set, b200mvs_plan_batches,
+ * b200mvs_optimize_patches and the sampling of neighbour views as they are, and add no device bytes (the mask travels
+ * in the batch's own map arrays).  It is not the clip of b200mvs_pset_clip_masks, which deletes points afterwards.
+ * The mask is copied; NULL clears it (w and h are then ignored).  Plans and pyramids are kept, and it works in a
+ * planning context, where it only stores the mask.  A bad view id, or w or h < 1 with a mask: B200MVS_ERR_INVALID_ARG. */
+int b200mvs_set_view_mask(b200mvs_ctx* ctx, int view_id, const uint8_t* mask_or_null, int w, int h);
 /* mve::Bundle::Features (bundle.h:51-60) as position + CSR list of referencing view ids. */
 int b200mvs_set_features(b200mvs_ctx* ctx, int n_features, const float* pos,
                          const int32_t* ref_offsets, const int32_t* ref_view_ids);

@@ -48,6 +48,8 @@ struct HostView {
     int w = 0, h = 0;
     float flen = 0, paspect = 1, pp[2] = {0.5f, 0.5f}, rot[9], trans[3];
     float k2 = 0, k4 = 0;          // radial distortion of the images it is given (b200mvs_set_view_distortion)
+    std::vector<uint8_t> mask;     // reconstruction mask, mask_w x mask_h, 0 = background (b200mvs_set_view_mask); empty: none
+    int mask_w = 0, mask_h = 0;
     float campos[3];
     float w2c[12];
     std::vector<HostLevel> lv;
@@ -62,6 +64,28 @@ size_t pyramid_bytes(const HostView& v)
     size_t texels = 0;
     for (const HostLevel& L : v.lv) texels += (size_t)L.pitch * L.h;
     return texels * (sizeof(uchar4) + sizeof(uint4));
+}
+
+// b200mvs_set_view_mask: the mask column (row) under the centre of column (row) x of a map n pixels wide (high), for a
+// mask m pixels wide (high): floor((2x+1) m / 2n)
+int mask_coord(int x, int n, int m) { return (int)((2ll * x + 1) * m / (2ll * n)); }
+// whether pixel (x, y) of view v's W x H map is background; a pixel outside the map is not
+bool background(const HostView& v, int W, int H, int x, int y)
+{
+    if (v.mask.empty() || x < 0 || y < 0 || x >= W || y >= H) return false;
+    return v.mask[(size_t)mask_coord(y, H, v.mask_h) * v.mask_w + mask_coord(x, W, v.mask_w)] == 0;
+}
+// bg[y * W + x] = 1 where pixel (x, y) of view v's W x H map is background, else 0 (v has a mask)
+void mark_background(const HostView& v, int W, int H, unsigned char* bg)
+{
+    std::vector<int> col(W);
+    for (int x = 0; x < W; ++x) col[x] = mask_coord(x, W, v.mask_w);
+    for (int y = 0; y < H; ++y) {
+        const uint8_t* row = v.mask.data() + (size_t)mask_coord(y, H, v.mask_h) * v.mask_w;
+        unsigned char* out = bg + (size_t)y * W;
+        if (v.mask_w == W) for (int x = 0; x < W; ++x) out[x] = row[x] == 0;          // col[x] == x: no gather
+        else for (int x = 0; x < W; ++x) out[x] = row[col[x]] == 0;
+    }
 }
 
 struct SeedPoint { int x, y; float depth; };
@@ -778,6 +802,24 @@ __global__ void k_slots_to_ids(const JobParams job, int32_t* __restrict__ out, b
     int32_t* o = out + 4 * p;
     if (aligned16) *reinterpret_cast<int4*>(o) = make_int4(ids[0], ids[1], ids[2], ids[3]);
     else { o[0] = ids[0]; o[1] = ids[1]; o[2] = ids[2]; o[3] = ids[3]; }
+}
+
+// Reconstruction masks (b200mvs_set_view_mask).  For the whole frontier launch a background pixel holds conf = +inf, which
+// no confidence (<= 1) passes: the stale test drops an entry of it, the commit test (old < conf) never writes it and the
+// push rule (c < conf - 0.05 || c == 0) never queues it, in k_frontier and k_frontier_resume alike.  `bg` has one byte per
+// pixel of the batch, nonzero = background; it lies in scratch map memory and is cleared as it is read.
+__global__ void k_mask_background(float* __restrict__ conf, unsigned char* __restrict__ bg, size_t n)
+{
+    const size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= n || !bg[p]) return;
+    bg[p] = 0;
+    conf[p] = INFINITY;
+}
+// after the launch: background pixels leave the device as unfilled ones, conf = 0
+__global__ void k_unmask_background(float* __restrict__ conf, size_t n)
+{
+    const size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (p < n && isinf(conf[p])) conf[p] = 0.f;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1898,6 +1940,19 @@ int b200mvs_set_view_distortion(b200mvs_ctx* ctx, int id, float k2, float k4)
     return 0;
 }
 
+int b200mvs_set_view_mask(b200mvs_ctx* ctx, int id, const uint8_t* mask, int w, int h)
+{
+    if (!ctx) return B200MVS_ERR_INVALID_ARG;
+    std::lock_guard<std::mutex> lk(ctx->mtx);
+    if (id < 0 || id >= (int)ctx->views.size() || (mask && (w < 1 || h < 1)))
+        return fail(B200MVS_ERR_INVALID_ARG, "b200mvs_set_view_mask: bad arguments");
+    HostView& v = ctx->views[id];
+    if (!mask) { v.mask.clear(); v.mask.shrink_to_fit(); v.mask_w = v.mask_h = 0; return 0; }
+    v.mask.assign(mask, mask + (size_t)w * h);
+    v.mask_w = w; v.mask_h = h;
+    return 0;
+}
+
 int b200mvs_set_features(b200mvs_ctx* ctx, int n, const float* pos, const int32_t* off, const int32_t* ids)
 {
     if (!ctx) return B200MVS_ERR_INVALID_ARG;
@@ -2581,6 +2636,7 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
     std::vector<Entry> seeds;
     size_t total_px = 0, n_tiles = 0;
     std::vector<size_t> px_off(n_refs);
+    bool masked = false;                   // a view of the group has a reconstruction mask
     for (int k = 0; k < n_refs; ++k) {
         const int j = js[k];
         jobs[k] = make_job(ctx, *s, refs[j], plans[j].gsel);
@@ -2589,7 +2645,10 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
         jobs[k].tiles_x = (jobs[k].W + 15) / 16;
         jobs[k].tile_base = (long long)n_tiles;
         n_tiles += (size_t)jobs[k].tiles_x * ((jobs[k].H + 15) / 16);
+        const HostView& rv = ctx->views[refs[j]];
+        masked = masked || !rv.mask.empty();
         for (const Seed& q : plans[j].seeds) {
+            if (background(rv, jobs[k].W, jobs[k].H, q.x, q.y)) continue;
             // a seed outside the image fails in the PatchSampler ctor (patch_sampler.cc:47-50); keep it so that the
             // processed count matches, the kernel rejects it by the same bounds test
             const int x = std::min(std::max(q.x, -1), 0xFFFE), y = std::min(std::max(q.y, -1), 0xFFFE);
@@ -2606,11 +2665,12 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
                         (unsigned long long)workspace_bytes(ctx, W), n_refs, cudaGetErrorString(e));
     }
     unsigned char* base = ctx->maps.p;
+    // sel first (8-byte alignment), then the float maps
+    float* const conf = reinterpret_cast<float*>(base + total_px * 8) + total_px;
+    const unsigned mask_blocks = (unsigned)((total_px + 255) / 256);
     {
-        // sel first (8-byte alignment), then the float maps
         unsigned long long* sel = reinterpret_cast<unsigned long long*>(base);
-        float* depth = reinterpret_cast<float*>(base + total_px * 8);
-        float* conf = depth + total_px;
+        float* depth = conf - total_px;
         float* dz = conf + total_px;
         float* normal = dz + 2 * total_px;
         unsigned* slots = reinterpret_cast<unsigned*>(normal + 3 * total_px);
@@ -2624,6 +2684,22 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
         }
         CK(cudaMemsetAsync(base, 0, total_px * (MAP_BYTES_PER_PX - 4), st));               // sel, depth, conf, dz, normal = 0
         CK(cudaMemsetAsync(slots, 0xFF, total_px * 4, st));
+        if (masked) {
+            // the background bytes of the masked views travel in the zeroed normal maps (12 bytes per pixel, one used),
+            // so a mask adds no device memory; k_mask_background zeroes them again
+            unsigned char* bg_dev = reinterpret_cast<unsigned char*>(normal);
+            std::vector<unsigned char> bg;
+            for (int k = 0; k < n_refs; ++k) {
+                const HostView& rv = ctx->views[refs[js[k]]];
+                if (rv.mask.empty()) continue;
+                bg.resize((size_t)jobs[k].W * jobs[k].H);
+                mark_background(rv, jobs[k].W, jobs[k].H, bg.data());
+                // pageable source: the call returns once `bg` has been read, so it may be refilled
+                CK(cudaMemcpyAsync(bg_dev + px_off[k], bg.data(), bg.size(), cudaMemcpyHostToDevice, st));
+            }
+            k_mask_background<<<mask_blocks, 256, 0, st>>>(conf, bg_dev, total_px);
+            CK(cudaGetLastError());
+        }
     }
     size_t cap = W.cap();
     const bool thresholded = W.thresholded;
@@ -2721,6 +2797,10 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
         P.n_seeds = 0;
     }
     ctx->fr_final = std::max<uint64_t>(ctx->fr_final, cap);
+    if (masked) {
+        k_unmask_background<<<mask_blocks, 256, 0, st>>>(conf, total_px);
+        CK(cudaGetLastError());
+    }
     if (progress) for (int k = 0; k < n_refs; ++k) if (progress[js[k]].cancelled) job_cancelled[k] = 1;
     const bool cancelled = h_ctl->stop == ST_CANCELLED || std::all_of(job_cancelled.begin(), job_cancelled.end(), [](char c) { return c != 0; });
     if (ctx->h_counters->count[C_OVERFLOW] || h_ctl->stop == ST_OVERFLOW)
@@ -2804,7 +2884,12 @@ int reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const i
             for (int g : plans[j].gsel)
                 if (!ctx->views[g].has_image) { if (failed_view) *failed_view = refs[j]; return fail(B200MVS_ERR_INVALID_ARG, "color image of view %d (selected neighbour of view %d) is not loaded", g, refs[j]); }
         }
-    if (stats) for (const HostPlan& p : plans) stats->n_seeds_processed += p.seeds.size();
+    if (stats)
+        for (int j = 0; j < n_refs; ++j) {
+            const HostView& rv = ctx->views[refs[j]];
+            const HostLevel& L = rv.lv[s->scale];
+            for (const Seed& q : plans[j].seeds) stats->n_seeds_processed += !background(rv, L.w, L.h, q.x, q.y);
+        }
     CK(cudaSetDevice(ctx->device));
 
     // ---- groups that fit the budget, one frontier launch each ----

@@ -86,7 +86,7 @@ EXPORTS = ["b200mvs_default_settings", "b200mvs_create", "b200mvs_destroy", "b20
            "b200mvs_pset_add_view", "b200mvs_pset_clip_masks", "b200mvs_pset_get_info", "b200mvs_pset_read",
            "b200mvs_pset_read_correspondence", "b200mvs_pset_add_reconstruction", "b200mvs_reconstruct_device",
            "b200mvs_get_level_device", "b200mvs_pset_add_view_device", "b200mvs_pset_create_on_device", "b200mvs_pset_read_device",
-           "b200mvs_set_view_distortion", "b200mvs_set_image_source_device"]
+           "b200mvs_set_view_distortion", "b200mvs_set_image_source_device", "b200mvs_set_view_mask"]
 
 ERR_INVALID_ARG = -1
 ERR_CUDA = -2
@@ -199,6 +199,7 @@ def lib():
                                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.b200mvs_set_features.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     L.b200mvs_set_view_distortion.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_float]
+    L.b200mvs_set_view_mask.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int]
     L.b200mvs_set_view_camera.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
     L.b200mvs_num_levels.argtypes = [C.c_void_p, C.c_int]
     L.b200mvs_get_level.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -417,6 +418,25 @@ class Scene:
         imports images unchanged.  A changed value drops the view's resident pyramid; cameras are unchanged."""
         self._check(self._lib.b200mvs_set_view_distortion(self._h, view_id, float(k2), float(k4)))
 
+    def set_view_mask(self, view_id: int, mask):
+        """Reconstruction mask of a reference view (b200mvs_set_view_mask): an H x W uint8 array, 0 = background, the
+        convention of scene2pset -m; a numpy array or a torch tensor (a CUDA tensor is copied to the host).  None clears it.
+        reconstruct(), reconstruct(on_device=True) and reconstruct_pointset() then never seed, queue or optimise a
+        background pixel: it ends unfilled (depth, conf, dz, normal 0, view ids -1) and yields no point.  Pixel (x, y) of a
+        W x H map is background when mask pixel ((2x+1) * mask_w // 2W, (2y+1) * mask_h // 2H) is 0, so the mask may have
+        the photo's size or any level's.  This differs from the `masks=` of reconstruct_pointset(), which deletes points of
+        the finished point set (scene2pset -m) after every pixel has been reconstructed."""
+        if mask is None:
+            self._check(self._lib.b200mvs_set_view_mask(self._h, view_id, None, 0, 0))
+            return
+        if hasattr(mask, "detach"):                  # a torch tensor, on the host or a device
+            mask = mask.detach().cpu().numpy()
+        m = np.asarray(mask)
+        if m.ndim != 2 or m.dtype != np.uint8:
+            raise ValueError("a view mask is an H x W uint8 array, not %s %s" % (m.dtype, m.shape))
+        m = np.ascontiguousarray(m)
+        self._check(self._lib.b200mvs_set_view_mask(self._h, view_id, _p(m), m.shape[1], m.shape[0]))
+
     def set_features(self, pos: np.ndarray, refs: Sequence[np.ndarray]):
         """mve::Bundle::Features (bundle.h:51-60)."""
         off = np.zeros(len(refs) + 1, np.int32)
@@ -606,7 +626,8 @@ class Scene:
                              on_device: bool = False):
         """DMRecon::start for a batch of reference views and scene2pset of their maps, without the maps leaving the device
         (b200mvs_pset_add_reconstruction).  options / masks / on_device: as for mve_b200.depthmap.scene_pointset (the masks
-        are applied after the reconstruction; on_device keeps the point set on the device and returns CUDA tensors);
+        are applied after the reconstruction, unlike set_view_mask, which keeps background pixels from being reconstructed
+        at all; on_device keeps the point set on the device and returns CUDA tensors);
         progress: as for reconstruct().  Returns (the dict of depthmap.scene_pointset, Stats)."""
         from . import depthmap
         return depthmap.reconstruct_pointset(self, settings, ref_views, options, masks, progress, on_device)

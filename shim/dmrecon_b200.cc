@@ -74,6 +74,7 @@ struct DeviceCtx {
     std::map<int, mve::ByteImage::Ptr> held;   // images the library fetched and has not released yet (image source)
     bool features_set = false;
     bool cameras_set = false;
+    std::vector<char> masks_set;    // views whose B200MVS_RECON_MASK embedding has been read
     bool leader_active = false;
     int planners = 0;               // callers that run their global view selection right now and will enqueue next
     std::vector<Request*> pending;
@@ -155,6 +156,29 @@ bool undistort_images()
 {
     const char* e = std::getenv("B200MVS_UNDISTORT");
     return e != nullptr && std::strcmp(e, "0") != 0 && *e != '\0';
+}
+
+// B200MVS_RECON_MASK=<embedding>: each reference view's one-channel image of that embedding is its reconstruction mask
+// (b200mvs_set_view_mask, 0 = background); unset or empty, views are reconstructed whole.
+const char* recon_mask_embedding()
+{
+    const char* e = std::getenv("B200MVS_RECON_MASK");
+    return e != nullptr && *e != '\0' ? e : nullptr;
+}
+
+// Reads view `id`'s mask embedding into the context.  A view without it, or with more than one channel, is reconstructed
+// unmasked, with the message scene2pset prints when it skips such a view (apps/scene2pset/scene2pset.cc:419-430).
+void set_recon_mask(b200mvs_ctx* ctx, mve::View::Ptr view, int id, const char* embedding)
+{
+    mve::ByteImage::Ptr mask = view->get_byte_image(embedding);
+    const char* problem = mask == nullptr ? "Mask not found for image \"" : mask->channels() != 1 ? "Expected 1-channel mask for image \"" : nullptr;
+    if (problem) {
+        std::lock_guard<std::mutex> lk(g_cout);
+        std::cout << problem << view->get_name() << "\", skipping." << std::endl;
+        return;
+    }
+    const int rc = b200mvs_set_view_mask(ctx, id, mask->get_data_pointer(), mask->width(), mask->height());
+    if (rc != 0) throw_for(rc, b200mvs_last_error(ctx));
 }
 
 // Device budget of a context: B200MVS_DEVICE_BUDGET_MB, or 0 = 90 % of the free device memory (include/b200mvs.h).
@@ -307,6 +331,7 @@ DMRecon::start()
         D.scene = scene;
         D.embedding = settings.imageEmbedding;
         D.held.clear();
+        D.masks_set.assign(mve_views.size(), 0);
         rc = b200mvs_set_image_source(D.ctx, fetch_image, release_image, &D, device_budget());
         if (rc != 0) throw std::runtime_error(b200mvs_last_error(D.ctx));
         set_frontier_capacity(D.ctx);
@@ -392,8 +417,19 @@ DMRecon::start()
        The result is parked in the context (b200mvs_plan_views); the leader's b200mvs_global_view_selection and
        b200mvs_reconstruct pick it up instead of computing it again. */
     progress.status = RECON_GLOBALVS;
+    const char* mask_embedding = recon_mask_embedding();
+    const bool read_mask = mask_embedding != nullptr && !D.masks_set[req.ref];
+    if (read_mask) D.masks_set[req.ref] = 1;
     D.planners++;
     lock.unlock();
+    try {
+        if (read_mask) set_recon_mask(ctx, mve_views[req.ref], req.ref, mask_embedding);
+    } catch (...) {
+        lock.lock();
+        D.planners--;
+        D.cv.notify_all();
+        throw;
+    }
     b200mvs_plan_views(ctx, &s, 1, &req.ref);        // a failure shows up again, with its message, in the leader's call
     lock.lock();
     D.planners--;
