@@ -363,12 +363,32 @@ void drop_pyramid(b200mvs_ctx* ctx, HostView& v)
     ctx->views_dirty = true;
 }
 
+// Whether the running call needs view v's pyramid (pin_views): it is never evicted
+bool pinned(const b200mvs_ctx* ctx, size_t v) { return v < ctx->pinned.size() && ctx->pinned[v]; }
+
+// Bytes of the resident pyramids that evict_lru may drop
+uint64_t evictable_bytes(const b200mvs_ctx* ctx)
+{
+    uint64_t b = 0;
+    for (size_t v = 0; v < ctx->views.size(); ++v)
+        if (ctx->views[v].d_base && !pinned(ctx, v)) b += ctx->views[v].bytes;
+    return b;
+}
+
+// Device bytes the running call may still allocate, keeping `reserve` free, when every evictable pyramid is dropped
+uint64_t headroom(const b200mvs_ctx* ctx, uint64_t reserve)
+{
+    if (!ctx->mem.budget) return UINT64_MAX;
+    const uint64_t limit = ctx->mem.budget + evictable_bytes(ctx);
+    return limit > ctx->mem.resident + reserve ? limit - ctx->mem.resident - reserve : 0;
+}
+
 bool evict_lru(b200mvs_ctx* ctx)
 {
     HostView* lru = nullptr;
     for (size_t i = 0; i < ctx->views.size(); ++i) {
         HostView& v = ctx->views[i];
-        if (!v.d_base || (i < ctx->pinned.size() && ctx->pinned[i])) continue;
+        if (!v.d_base || pinned(ctx, i)) continue;
         if (!lru || v.last_use < lru->last_use) lru = &v;
     }
     if (!lru) return false;
@@ -2321,18 +2341,11 @@ int plan_on_device(b200mvs_ctx* ctx, const b200mvs_settings& s, const int32_t* r
         const uint64_t words = PL::job_layout(J.F, J.E, nv, nf).words + PL::out_words(J.seed_cap) + sizeof(PL::PlanJob) / 4;
         jobs.push_back(Sized{j, J, (size_t)words * 4});
     }
-    // what the call may hold: the budget, less what stays resident (pyramids of unpinned views can be evicted); without a
-    // budget, half the free device memory
-    const uint64_t limit = budget_limit(ctx);
-    if (ctx->mem.budget && ctx->mem.resident + in_bytes + jobs[0].bytes > limit) release_workspace(ctx);
-    uint64_t avail;
-    if (ctx->mem.budget) {
-        uint64_t evictable = 0;
-        for (size_t v = 0; v < ctx->views.size(); ++v)
-            if (ctx->views[v].d_base && !(v < ctx->pinned.size() && ctx->pinned[v])) evictable += ctx->views[v].bytes;
-        const uint64_t held = ctx->mem.resident - evictable;
-        avail = limit > held ? limit - held : 0;
-    } else {
+    // what the call may hold: the budget's headroom (pyramids of unpinned views can be evicted); without a budget, half
+    // the free device memory
+    if (ctx->mem.budget && ctx->mem.resident + in_bytes + jobs[0].bytes > ctx->mem.budget) release_workspace(ctx);
+    uint64_t avail = headroom(ctx, 0);
+    if (!ctx->mem.budget) {
         size_t free_b = 0, total_b = 0;
         CK(cudaMemGetInfo(&free_b, &total_b));
         avail = free_b / 2;
@@ -2534,14 +2547,7 @@ int plan_groups(b200mvs_ctx* ctx, const b200mvs_settings& s, int n, const int32_
 int grow_frontier(b200mvs_ctx* ctx, const FrontierCtl& c, FrontierParams& P, size_t& cap, uint64_t reserve)
 {
     const uint64_t need = c.need;
-    uint64_t room = UINT64_MAX;
-    if (ctx->mem.budget) {
-        uint64_t evictable = 0;                  // pyramids make_room may drop: those the group does not need
-        for (size_t i = 0; i < ctx->views.size(); ++i)
-            if (ctx->views[i].d_base && !(i < ctx->pinned.size() && ctx->pinned[i])) evictable += ctx->views[i].bytes;
-        const uint64_t limit = ctx->mem.budget + evictable;
-        room = limit > ctx->mem.resident + reserve ? limit - ctx->mem.resident - reserve : 0;
-    }
+    const uint64_t room = headroom(ctx, reserve);   // the pyramids the group does not need may be evicted
     auto extra = [&](uint64_t n) {              // accounted bytes the frontier arrays add at n entries
         uint64_t b = 0;
         for_each_frontier_array(ctx, [&](auto& buf) { if (n > buf.cap) b += (n - buf.cap) * sizeof(*buf.p); });
@@ -2581,20 +2587,22 @@ int grow_frontier(b200mvs_ctx* ctx, const FrontierCtl& c, FrontierParams& P, siz
     return 0;
 }
 
-// Where b200mvs_pset_add_reconstruction and b200mvs_reconstruct_device send the maps instead of host buffers.  take(j, job) runs for every view of a group
-// that was not cancelled, right after the group's launch, while the group's maps and pyramids are resident; it may
-// allocate up to bytes(w, h) device bytes for a map of w x h pixels through the accounted allocator, and every group's plan
-// keeps that much free for the largest map of the batch.
+// Where a reconstruction's maps go: the caller's buffers (buffer_sink) or a point set.  Right after a group's launch,
+// unless the whole group was cancelled, each view j gets its width and height in sizes[j] (when set) and, unless it was
+// cancelled, take(j, job) runs while the group's maps and pyramids are resident.  take may allocate up to bytes(w, h)
+// device bytes for a map of w x h pixels through the accounted allocator; every group's plan keeps that much free for
+// the largest map of the batch.
 struct MapSink {
     std::function<uint64_t(int w, int h)> bytes;
     std::function<int(int j, const JobParams& job)> take;
+    b200mvs_maps* sizes = nullptr;
 };
 
 // One frontier launch over the reference views refs[j], j in js (at most MAX_GROUP_VIEWS): makes room for the pyramids
-// they need within the budget (`reserve` bytes kept free for the sink), loads the missing ones, runs.  Accumulates
-// `stats`; marks the views that ended cancelled in `view_cancelled`.
+// they need within the budget (`reserve` bytes kept free for the sink), loads the missing ones, runs, hands the maps to
+// `sink`.  Accumulates `stats`; marks the views that ended cancelled in `view_cancelled`.
 int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int>& js, const int32_t* refs,
-              const std::vector<HostPlan>& plans, b200mvs_maps* maps, const MapSink* sink, uint64_t reserve,
+              const std::vector<HostPlan>& plans, const MapSink* sink, uint64_t reserve,
               b200mvs_progress* progress, b200mvs_stats* stats, int32_t* failed_view, std::vector<char>& view_cancelled)
 {
     // `if (progress.cancelled) return` at the head of every stage (dmrecon.cc:100-104,336): a group whose views were all
@@ -2808,30 +2816,14 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
     if (stats) stats->n_seeds_success += ctx->h_counters->count[C_SEED_OK];
 
     // ---- results ----
-    if ((maps || sink) && !cancelled) {
-        std::vector<unsigned> hslots;
+    if (sink && !cancelled)
         for (int k = 0; k < n_refs; ++k) {
             const int j = js[k];
-            const size_t np = (size_t)jobs[k].W * jobs[k].H;
-            if (maps) { maps[j].width = jobs[k].W; maps[j].height = jobs[k].H; }
+            if (sink->sizes) { sink->sizes[j].width = jobs[k].W; sink->sizes[j].height = jobs[k].H; }
             if (job_cancelled[k]) continue;                  // RECON_CANCELLED: nothing is saved (dmrecon.cc:100-104)
             if (progress) progress[j].status = 4;
-            if (sink) {
-                if ((rc = sink->take(j, jobs[k]))) { if (failed_view) *failed_view = refs[j]; return rc; }
-                continue;
-            }
-            if (maps[j].depth) CK(cudaMemcpyAsync(maps[j].depth, jobs[k].depth, np * 4, cudaMemcpyDeviceToHost, st));
-            if (maps[j].conf) CK(cudaMemcpyAsync(maps[j].conf, jobs[k].conf, np * 4, cudaMemcpyDeviceToHost, st));
-            if (maps[j].dz) CK(cudaMemcpyAsync(maps[j].dz, jobs[k].dz, np * 8, cudaMemcpyDeviceToHost, st));
-            if (maps[j].normal) CK(cudaMemcpyAsync(maps[j].normal, jobs[k].normal, np * 12, cudaMemcpyDeviceToHost, st));
-            if (maps[j].view_ids) {
-                hslots.resize(np);
-                CK(cudaMemcpyAsync(hslots.data(), jobs[k].slots, np * 4, cudaMemcpyDeviceToHost, st));
-                CK(cudaStreamSynchronize(st));
-                for (size_t p = 0; p < np; ++p) slots_to_ids(jobs[k].gview, jobs[k].n_global, hslots[p], maps[j].view_ids + 4 * p);
-            }
+            if ((rc = sink->take(j, jobs[k]))) { if (failed_view) *failed_view = refs[j]; return rc; }
         }
-    }
     CK(cudaStreamSynchronize(st));
     uint64_t filled = 0;
     for (int k = 0; k < n_refs; ++k) {
@@ -2862,11 +2854,11 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
     return 0;
 }
 
-// b200mvs_reconstruct with the context locked and a device: without a sink the maps go to `maps` (NULL: stay on the
-// device, one group only); with one, each view's maps go to the sink after its group's launch and no group plans into
-// the sink's bytes for the largest map of the batch (`maps`, when given, still receives every width and height).
-int reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* refs, b200mvs_maps* maps,
-                const MapSink* sink, b200mvs_progress* progress, b200mvs_stats* stats, int32_t* failed_view)
+// A reconstruction with the context locked and a device: each view's maps go to the sink after its group's launch, and no
+// group plans into the sink's bytes for the largest map of the batch; without a sink they stay on the device, one group
+// only.
+int reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* refs, const MapSink* sink,
+                b200mvs_progress* progress, b200mvs_stats* stats, int32_t* failed_view)
 {
     // without a budget the whole batch is one launch; with one, the limit applies per group
     if (!ctx->mem.budget && n_refs > MAX_GROUP_VIEWS) return fail(B200MVS_ERR_INVALID_ARG, "b200mvs_reconstruct: bad arguments");
@@ -2903,19 +2895,49 @@ int reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const i
     std::vector<int> group_of;
     const int n_groups = plan_groups(ctx, *s, n_refs, refs, plans, limit > fixed + reserve ? limit - fixed - reserve : 0, group_of, failed_view);
     if (n_groups < 0) return n_groups;
-    if (!maps && !sink && n_groups > 1)
+    if (!sink && n_groups > 1)
         return fail(B200MVS_ERR_INVALID_ARG, "maps == NULL keeps the results on the device, but the budget splits the batch into %d launches", n_groups);
     ctx->mem.n_groups = (uint64_t)n_groups;
     std::vector<char> view_cancelled(n_refs, 0);
     for (int g = 0; g < n_groups; ++g) {
         std::vector<int> js;
         for (int j = 0; j < n_refs; ++j) if (group_of[j] == g) js.push_back(j);
-        if ((rc = run_group(ctx, s, js, refs, plans, maps, sink, reserve, progress, stats, failed_view, view_cancelled))) return rc;
+        if ((rc = run_group(ctx, s, js, refs, plans, sink, reserve, progress, stats, failed_view, view_cancelled))) return rc;
     }
     ctx->pinned.clear();
     if (std::all_of(view_cancelled.begin(), view_cancelled.end(), [](char c) { return c != 0; }))
         return fail(B200MVS_ERR_CANCELLED, "reconstruction cancelled");
     return 0;
+}
+
+// The sink into the caller's buffers `maps` (host memory, or with on_device the context's device): copies on ctx->stream,
+// view ids decoded on the host or by k_slots_to_ids.  The buffers are not the context's, so it reserves no budget.
+MapSink buffer_sink(b200mvs_ctx* ctx, b200mvs_maps* maps, bool on_device)
+{
+    MapSink sink;
+    sink.sizes = maps;
+    sink.bytes = [](int, int) { return (uint64_t)0; };
+    sink.take = [ctx, maps, on_device, hslots = std::vector<unsigned>()](int j, const JobParams& J) mutable {
+        const b200mvs_maps& m = maps[j];
+        const size_t np = (size_t)J.W * J.H;
+        const cudaStream_t st = ctx->stream;
+        const cudaMemcpyKind kind = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+        if (m.depth) CK(cudaMemcpyAsync(m.depth, J.depth, np * 4, kind, st));
+        if (m.conf) CK(cudaMemcpyAsync(m.conf, J.conf, np * 4, kind, st));
+        if (m.dz) CK(cudaMemcpyAsync(m.dz, J.dz, np * 8, kind, st));
+        if (m.normal) CK(cudaMemcpyAsync(m.normal, J.normal, np * 12, kind, st));
+        if (m.view_ids && on_device) {
+            k_slots_to_ids<<<(unsigned)((np + 255) / 256), 256, 0, st>>>(J, m.view_ids, reinterpret_cast<uintptr_t>(m.view_ids) % 16 == 0);
+            CK(cudaGetLastError());
+        } else if (m.view_ids) {
+            hslots.resize(np);
+            CK(cudaMemcpyAsync(hslots.data(), J.slots, np * 4, cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
+            for (size_t p = 0; p < np; ++p) slots_to_ids(J.gview, J.n_global, hslots[p], m.view_ids + 4 * p);
+        }
+        return 0;
+    };
+    return sink;
 }
 
 } // namespace
@@ -2929,7 +2951,9 @@ int b200mvs_reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs,
     std::lock_guard<std::mutex> lk(ctx->mtx);
     int rc = require_device(ctx);
     if (rc) return rc;
-    return reconstruct(ctx, s, n_refs, refs, maps, nullptr, progress, stats, failed_view);
+    if (!maps) return reconstruct(ctx, s, n_refs, refs, nullptr, progress, stats, failed_view);
+    const MapSink sink = buffer_sink(ctx, maps, false);
+    return reconstruct(ctx, s, n_refs, refs, &sink, progress, stats, failed_view);
 }
 
 int b200mvs_reconstruct_device(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* refs, b200mvs_maps* maps_dev,
@@ -2953,26 +2977,8 @@ int b200mvs_reconstruct_device(b200mvs_ctx* ctx, const b200mvs_settings* s, int 
             if (b.first && (rc = check_device_buffer(fn, what(b.second), b.first, ctx->device, 4))) return rc;
     }
     if ((rc = wait_for_caller(ctx, cuda_stream))) return rc;
-    // each view's maps go straight from the group's map arrays into the caller's buffers, on ctx->stream right after the
-    // group's launch; the caller's buffers are not the context's, so the sink reserves nothing in the budget
-    MapSink sink;
-    sink.bytes = [](int, int) { return (uint64_t)0; };
-    sink.take = [&](int j, const JobParams& J) {
-        const b200mvs_maps& m = maps_dev[j];
-        const size_t np = (size_t)J.W * J.H;
-        const cudaStream_t st = ctx->stream;
-        CK(cudaMemcpyAsync(m.depth, J.depth, np * 4, cudaMemcpyDeviceToDevice, st));
-        if (m.conf) CK(cudaMemcpyAsync(m.conf, J.conf, np * 4, cudaMemcpyDeviceToDevice, st));
-        if (m.dz) CK(cudaMemcpyAsync(m.dz, J.dz, np * 8, cudaMemcpyDeviceToDevice, st));
-        if (m.normal) CK(cudaMemcpyAsync(m.normal, J.normal, np * 12, cudaMemcpyDeviceToDevice, st));
-        if (m.view_ids) {
-            k_slots_to_ids<<<(unsigned)((np + 255) / 256), 256, 0, st>>>(J, m.view_ids, reinterpret_cast<uintptr_t>(m.view_ids) % 16 == 0);
-            CK(cudaGetLastError());
-        }
-        return 0;
-    };
-    // maps_dev also goes in as `maps`, which receives each view's width and height as b200mvs_reconstruct's maps do
-    return reconstruct(ctx, s, n_refs, refs, maps_dev, &sink, progress, stats, failed_view);
+    const MapSink sink = buffer_sink(ctx, maps_dev, true);
+    return reconstruct(ctx, s, n_refs, refs, &sink, progress, stats, failed_view);
 }
 
 int b200mvs_pset_add_reconstruction(b200mvs_pset* ps, b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* refs,
@@ -3003,7 +3009,7 @@ int b200mvs_pset_add_reconstruction(b200mvs_pset* ps, b200mvs_ctx* ctx, const b2
         return rc ? fail(rc, "view %d: %s", refs[j], b200mvs_depthmap_last_error()) : 0;
     };
     PD::use_allocator(ps, &A);
-    const int rc = reconstruct(ctx, s, n_refs, refs, nullptr, &sink, progress, stats, failed_view);
+    const int rc = reconstruct(ctx, s, n_refs, refs, &sink, progress, stats, failed_view);
     PD::use_allocator(ps, nullptr);
     if (rc) { PD::discard(ps); return rc; }
     if (int crc = PD::commit(ps, blocks, views_out)) return fail(crc, "%s", b200mvs_depthmap_last_error());
