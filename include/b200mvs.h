@@ -398,8 +398,8 @@ int b200mvs_plan_batches(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs
                          uint64_t available, int32_t* group_of_ref, int32_t* failed_view_or_null);
 
 /* ---- consumers of the depth maps, on the device (SURVEY.md 8f rank 2 and 3).  Stateless: host buffers in, host buffers
- *      out, `device` = CUDA device ordinal.  Errors: negative code, message from b200mvs_depthmap_last_error(). ---- */
-const char* b200mvs_depthmap_last_error(void);
+ *      out, `device` = CUDA device ordinal.  Errors: negative code, message from b200mvs_last_error(). ---- */
+const char* b200mvs_depthmap_last_error(void);   /* the same message as b200mvs_last_error */
 /* mve::image::depthmap_confidence_clean (libs/mve/depthmap.cc:118-131): depth = 0 where conf <= 0, in place. */
 int b200mvs_depthmap_confidence_clean(int device, float* depth, const float* conf, int w, int h);
 /* mve::image::depthmap_cleanup (depthmap.cc:25-113): 4-connected islands of depth != 0 smaller than thres pixels are erased. */
@@ -436,7 +436,7 @@ int b200mvs_depthmap_pointset(int device, const float* depth, int w, int h, cons
  * memory of a handle made by b200mvs_pset_create does not grow with the number of views or points: one view's workspace
  * (kept at the largest view added so far), plus the masks and one chunk of points during clipping.  A handle made by
  * b200mvs_pset_create_on_device keeps its point set in DEVICE memory instead (below).  Errors: negative code,
- * b200mvs_depthmap_last_error(). */
+ * b200mvs_last_error(). */
 typedef struct b200mvs_pset b200mvs_pset;
 typedef struct b200mvs_pset_options {
     int32_t with_normals;         /* -n: angle-weighted vertex normals                                              */

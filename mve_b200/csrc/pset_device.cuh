@@ -39,7 +39,7 @@ struct Allocator {
     void (*free)(void* user, void* p, size_t bytes) = nullptr;
 };
 
-// B200MVS_ERR_INVALID_ARG (message in b200mvs_depthmap_last_error) for a NULL handle, a handle on another device than
+// B200MVS_ERR_INVALID_ARG (message in b200mvs_last_error) for a NULL handle, a handle on another device than
 // `device` or one whose masks have been applied
 int check(const b200mvs_pset* ps, int device);
 // Device bytes the handle's workspace holds at most for one map of w x h pixels with a colour image
