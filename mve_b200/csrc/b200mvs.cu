@@ -18,6 +18,7 @@
 #include <cstdlib>
 #include <functional>
 #include <map>
+#include <memory>
 #include <chrono>
 #include <ctime>
 #include <mutex>
@@ -33,6 +34,54 @@ using namespace b200mvs_host;
 // small helpers
 // ------------------------------------------------------------------------------------------------
 namespace {
+
+// Every device allocation of a context goes through these two (defined after b200mvs_ctx): they keep the resident / peak
+// byte counts of b200mvs_memory_stats and make room within the budget first.
+cudaError_t dev_alloc(b200mvs_ctx* ctx, void** p, size_t bytes);
+void dev_free(b200mvs_ctx* ctx, void* p, size_t bytes);
+
+// A device buffer of context `ctx`, allocated through its accounted allocator and freed when it goes out of scope
+template <typename T> struct DevBuf {
+    b200mvs_ctx* ctx;
+    T* p = nullptr;
+    size_t cap = 0;
+    explicit DevBuf(b200mvs_ctx* c) : ctx(c) {}
+    DevBuf(DevBuf&& o) noexcept : ctx(o.ctx), p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+    ~DevBuf() { release(); }
+    size_t bytes() const { return cap * sizeof(T); }
+    cudaError_t reserve(size_t n)
+    {
+        if (n <= cap) return cudaSuccess;
+        release();
+        cudaError_t e = dev_alloc(ctx, reinterpret_cast<void**>(&p), n * sizeof(T));
+        if (e == cudaSuccess) cap = n;
+        return e;
+    }
+    void release() { dev_free(ctx, p, bytes()); p = nullptr; cap = 0; }
+    // grows to n elements keeping the first `keep`: the copy has finished before the old buffer is freed
+    cudaError_t grow(size_t n, size_t keep, cudaStream_t st)
+    {
+        if (n <= cap) return cudaSuccess;
+        if (keep == 0) return reserve(n);
+        T* q = nullptr;
+        cudaError_t e = dev_alloc(ctx, reinterpret_cast<void**>(&q), n * sizeof(T));
+        if (e != cudaSuccess) return e;
+        e = cudaMemcpyAsync(q, p, keep * sizeof(T), cudaMemcpyDeviceToDevice, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess) { dev_free(ctx, q, n * sizeof(T)); return e; }
+        release();
+        p = q; cap = n;
+        return cudaSuccess;
+    }
+};
+
+// Owners of the pinned host blocks, events and stream of a context
+struct FreeHost { void operator()(void* p) const { cudaFreeHost(p); } };
+struct DestroyEvent { void operator()(cudaEvent_t e) const { cudaEventDestroy(e); } };
+struct DestroyStream { void operator()(cudaStream_t s) const { cudaStreamDestroy(s); } };
+template <typename T> using Pinned = std::unique_ptr<T, FreeHost>;
+using Event = std::unique_ptr<CUevent_st, DestroyEvent>;
+using Stream = std::unique_ptr<CUstream_st, DestroyStream>;
 
 struct HostLevel {
     int w = 0, h = 0, pitch = 0;
@@ -52,9 +101,9 @@ struct HostView {
     float campos[3];
     float w2c[12];
     std::vector<HostLevel> lv;
-    uchar4* d_base = nullptr;      // one allocation for every level: the RGBX8 images, then their quad images
-    size_t bytes = 0;
+    DevBuf<uchar4> pyr;            // one allocation for every level: the RGBX8 images, then their quad images
     uint64_t last_use = 0;         // eviction order: least recently used first
+    explicit HostView(b200mvs_ctx* ctx) : pyr(ctx) {}
 };
 
 // Device bytes of a view's pyramid: every level of buildPyramid, RGBX8 + quad image (16 B) per texel at a pitch of 4 texels
@@ -160,6 +209,8 @@ struct HostMirror {                             // mapped pinned host memory; fo
 };                                              // ... and by cancel_job[n_jobs] (host -> device: drop this view's queue)
 
 constexpr int MAX_GROUP_VIEWS = 4000;           // reference views per frontier launch
+constexpr size_t MIRROR_BYTES = sizeof(HostMirror) + (sizeof(unsigned long long) + sizeof(int)) * MAX_GROUP_VIEWS;
+static_assert(sizeof(HostMirror) % alignof(unsigned long long) == 0, "filled[] follows the mirror, aligned");
 
 struct HostCounters {                           // pinned: what the host reads back after a launch
     unsigned long long count[C_NUM + MAX_GROUP_VIEWS];   // the Counter totals, then `filled` of every job of the group
@@ -167,40 +218,6 @@ struct HostCounters {                           // pinned: what the host reads b
 };
 static_assert(offsetof(HostCounters, ctl) >= sizeof(unsigned long long) * (C_NUM + MAX_GROUP_VIEWS),
               "the counters of a full group end before the control block");
-
-// Every device allocation of a context goes through these two (defined after b200mvs_ctx): they keep the resident / peak
-// byte counts of b200mvs_memory_stats and make room within the budget first.
-cudaError_t dev_alloc(b200mvs_ctx* ctx, void** p, size_t bytes);
-void dev_free(b200mvs_ctx* ctx, void* p, size_t bytes);
-
-template <typename T> struct DevBuf {
-    T* p = nullptr;
-    size_t cap = 0;
-    cudaError_t reserve(b200mvs_ctx* ctx, size_t n)
-    {
-        if (n <= cap) return cudaSuccess;
-        release(ctx);
-        cudaError_t e = dev_alloc(ctx, reinterpret_cast<void**>(&p), n * sizeof(T));
-        if (e == cudaSuccess) cap = n;
-        return e;
-    }
-    void release(b200mvs_ctx* ctx) { dev_free(ctx, p, cap * sizeof(T)); p = nullptr; cap = 0; }
-    // grows to n elements keeping the first `keep`: the copy has finished before the old buffer is freed
-    cudaError_t grow(b200mvs_ctx* ctx, size_t n, size_t keep, cudaStream_t st)
-    {
-        if (n <= cap) return cudaSuccess;
-        if (keep == 0) return reserve(ctx, n);
-        T* q = nullptr;
-        cudaError_t e = dev_alloc(ctx, reinterpret_cast<void**>(&q), n * sizeof(T));
-        if (e != cudaSuccess) return e;
-        e = cudaMemcpyAsync(q, p, keep * sizeof(T), cudaMemcpyDeviceToDevice, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) { dev_free(ctx, q, n * sizeof(T)); return e; }
-        release(ctx);
-        p = q; cap = n;
-        return cudaSuccess;
-    }
-};
 
 // Initial frontier capacity of a launch: max(ceil(per_px x pixels), seeds, min) entries (b200mvs_set_frontier_capacity).
 struct FrontierCapacity {
@@ -228,49 +245,65 @@ static_assert(sizeof(JobParams) == 232 && sizeof(PatchOut) == 40, "per-view and 
 
 } // namespace
 
+// Members are destroyed in reverse order: the accounting outlives every owner that updates it, the stream outlives the
+// buffers, and the device buffers go before the pinned blocks and events.  A planning context (B200MVS_DEVICE_NONE) owns
+// none of them, so destroying it makes no CUDA call.
 struct b200mvs_ctx {
     int device = 0;
-    cudaStream_t stream = nullptr;
+    // device memory accounting (dev_alloc), with the budget of the image source (b200mvs_set_image_source)
+    b200mvs_memory mem = {};
+    uint64_t pyr_resident = 0;         // part of mem.resident held by pyramids
+    Stream stream;
+    Event ev_begin, ev_end;            // the timing of a launch
+    Event ev_copied;                   // a frontier launch's counters and control block are on the host
+    Event ev_caller;                   // what a *_device call waits for on the caller's stream
+    Event ev_source;                   // a device source's image is ready, and later the pyramids built from it
+    Pinned<HostCounters> h_counters;
+    Pinned<HostMirror> h_mirror;       // mapped, MIRROR_BYTES
+    // b200mvs_upload_view staging: two slots used alternately, so that the host copy of view k+1 overlaps the H2D transfer
+    // and the pyramid kernels of view k (SURVEY 8f rank 1).  For a host image a slot holds a pinned host block and a device
+    // block; for a device image, read in place, it only charges the budget (next_stage).
+    struct Stage {
+        Pinned<uint8_t> host;
+        DevBuf<uint8_t> dev;
+        size_t charged = 0;            // bytes charged with dev_charge, without `dev`
+        Event done;
+        bool busy = false;
+        explicit Stage(b200mvs_ctx* ctx) : dev(ctx) {}
+        size_t cap() const { return dev.p ? dev.cap : charged; }
+    };
+    Stage stage[2] = {Stage(this), Stage(this)};
+    unsigned stage_next = 0;
     std::mutex mtx;
     std::vector<HostView> views;
     std::vector<HostFeature> feats;
     std::vector<std::vector<int>> view_feats;   // inverted index: ascending ids of the features that reference a view
-    ViewParams* d_views = nullptr;
+    DevBuf<ViewParams> d_views{this};
     bool views_dirty = true;
-    float* d_lut = nullptr;
+    DevBuf<float> d_lut{this};
     // workspace (grown on demand, reused across calls)
-    DevBuf<Entry> ent_a, ent_b, run_in, run_sorted;
-    DevBuf<unsigned> tile_cnt;
-    DevBuf<unsigned long long> tile_off;
-    DevBuf<PatchOut> run_out;
-    DevBuf<unsigned char> written;
-    DevBuf<unsigned long long> counters;
-    DevBuf<JobParams> d_jobs;
-    DevBuf<DevSettings> d_settings;
-    DevBuf<unsigned char> maps;        // all per-job maps of the current batch
-    DevBuf<FrontierCtl> ctl;
-    DevBuf<unsigned> hist;
-    DevBuf<int> thr_bin;
-    DevBuf<int> job_cancel;
-    DevBuf<unsigned long long> job_run;
+    DevBuf<Entry> ent_a{this}, ent_b{this}, run_in{this}, run_sorted{this};
+    DevBuf<unsigned> tile_cnt{this};
+    DevBuf<unsigned long long> tile_off{this};
+    DevBuf<PatchOut> run_out{this};
+    DevBuf<unsigned char> written{this};
+    DevBuf<unsigned long long> counters{this};
+    DevBuf<JobParams> d_jobs{this};
+    DevBuf<DevSettings> d_settings{this};
+    DevBuf<unsigned char> maps{this};  // all per-job maps of the current batch
+    DevBuf<FrontierCtl> ctl{this};
+    DevBuf<unsigned> hist{this};
+    DevBuf<int> thr_bin{this};
+    DevBuf<int> job_cancel{this};
+    DevBuf<unsigned long long> job_run{this};
     int frontier_grid = 0;             // CTAs of the cooperative launch (= what fits on the chip)
     int optimize_grid = 0;             // resident CTAs of k_optimize
     long long thread_min = -1;         // reconstruct: rounds with at least this many patches run one thread per patch (-1: default)
     int optimize_mode = 0;             // b200mvs_optimize_patches: 0 by batch size, 1 one warp per patch, 2 one thread per patch
-    HostCounters* h_counters = nullptr;
-    unsigned long long* h_mirror = nullptr;     // pinned + mapped: HostMirror
-    std::vector<cudaEvent_t> ev_pool;
-    // b200mvs_upload_view staging: two pinned host buffers + device buffers used alternately, so that the host copy of
-    // view k+1 overlaps the H2D transfer and the pyramid kernels of view k (SURVEY 8f rank 1)
-    struct Stage { uint8_t* host = nullptr; uint8_t* dev = nullptr; size_t cap = 0; cudaEvent_t done = nullptr; bool busy = false; };
-    Stage stage[2];
-    unsigned stage_next = 0;
     // host plans prepared ahead by b200mvs_plan_views (global view selection + seed list of a reference view)
     std::mutex plan_mtx;
     std::map<int, HostPlan> plans;
-    // device memory accounting and the optional image source (b200mvs_set_image_source)
-    b200mvs_memory mem = {};
-    uint64_t pyr_resident = 0;         // part of mem.resident held by pyramids
+    // pyramid eviction and the optional image source
     uint64_t use_clock = 0;
     b200mvs_fetch_fn fetch = nullptr;              // a host image source, or
     b200mvs_device_fetch_fn fetch_device = nullptr; // a device image source (at most one of the two is set)
@@ -283,6 +316,12 @@ struct b200mvs_ctx {
     b200mvs_plan_info plan_info = {};  // of the last b200mvs_reconstruct
     std::vector<float> plx_table;      // the device planner's parallax factors for min_parallax = plx_table_mp
     float plx_table_mp = -1.f;
+
+    b200mvs_ctx(int device_, int n_views) : device(device_)
+    {
+        views.reserve(n_views);
+        for (int i = 0; i < n_views; ++i) views.emplace_back(this);
+    }
 };
 
 namespace {
@@ -320,11 +359,11 @@ uint64_t workspace_grown_bytes(b200mvs_ctx* ctx, const Workspace& w)
 }
 void shrink_workspace(b200mvs_ctx* ctx, const Workspace& w)
 {
-    for_each_workspace(ctx, w, [&](auto& buf, size_t n) { if (buf.cap > n) buf.release(ctx); });
+    for_each_workspace(ctx, w, [&](auto& buf, size_t n) { if (buf.cap > n) buf.release(); });
 }
 void release_workspace(b200mvs_ctx* ctx)
 {
-    for_each_workspace(ctx, Workspace{}, [&](auto& buf, size_t) { buf.release(ctx); });
+    for_each_workspace(ctx, Workspace{}, [&](auto& buf, size_t) { buf.release(); });
 }
 
 // Allocations that do not depend on the batch: view table, sRGB table, settings, frontier control block and the two
@@ -343,9 +382,8 @@ uint64_t budget_limit(const b200mvs_ctx* ctx) { return ctx->mem.budget ? ctx->me
 
 void drop_pyramid(b200mvs_ctx* ctx, HostView& v)
 {
-    dev_free(ctx, v.d_base, v.bytes);
-    ctx->pyr_resident -= v.bytes;
-    v.d_base = nullptr; v.bytes = 0;
+    ctx->pyr_resident -= v.pyr.bytes();
+    v.pyr.release();
     v.has_image = false;
     for (HostLevel& L : v.lv) { L.d_img = nullptr; L.d_quad = nullptr; }
     ctx->views_dirty = true;
@@ -359,7 +397,7 @@ uint64_t evictable_bytes(const b200mvs_ctx* ctx)
 {
     uint64_t b = 0;
     for (size_t v = 0; v < ctx->views.size(); ++v)
-        if (ctx->views[v].d_base && !pinned(ctx, v)) b += ctx->views[v].bytes;
+        if (!pinned(ctx, v)) b += ctx->views[v].pyr.bytes();
     return b;
 }
 
@@ -376,7 +414,7 @@ bool evict_lru(b200mvs_ctx* ctx)
     HostView* lru = nullptr;
     for (size_t i = 0; i < ctx->views.size(); ++i) {
         HostView& v = ctx->views[i];
-        if (!v.d_base || pinned(ctx, i)) continue;
+        if (!v.pyr.p || pinned(ctx, i)) continue;
         if (!lru || v.last_use < lru->last_use) lru = &v;
     }
     if (!lru) return false;
@@ -408,6 +446,12 @@ void pin_views(b200mvs_ctx* ctx, const std::vector<int>& ids)
     for (int id : ids) if (id >= 0 && id < (int)ctx->pinned.size()) { ctx->pinned[id] = 1; ctx->views[id].last_use = ++ctx->use_clock; }
 }
 
+struct PinsOfCall {                             // the views an entry point pins are unpinned when the call returns
+    b200mvs_ctx* c;
+    explicit PinsOfCall(b200mvs_ctx* c_) : c(c_) {}
+    ~PinsOfCall() { c->pinned.assign(c->views.size(), 0); }
+};
+
 // The only cudaMalloc / cudaFree of the library (tests/test_device_budget.py checks the source).
 cudaError_t dev_alloc(b200mvs_ctx* ctx, void** p, size_t bytes)
 {
@@ -421,7 +465,7 @@ cudaError_t dev_alloc(b200mvs_ctx* ctx, void** p, size_t bytes)
     return cudaSuccess;
 }
 
-// Charges `bytes` to the budget as dev_alloc does, without allocating them
+// Charges `bytes` to the budget as dev_alloc does, without allocating them; dev_uncharge gives them back
 cudaError_t dev_charge(b200mvs_ctx* ctx, size_t bytes)
 {
     if (!make_room(ctx, bytes)) return cudaErrorMemoryAllocation;
@@ -429,6 +473,8 @@ cudaError_t dev_charge(b200mvs_ctx* ctx, size_t bytes)
     ctx->mem.peak = std::max(ctx->mem.peak, ctx->mem.resident);
     return cudaSuccess;
 }
+
+void dev_uncharge(b200mvs_ctx* ctx, size_t bytes) { ctx->mem.resident -= bytes; }
 
 void dev_free(b200mvs_ctx* ctx, void* p, size_t bytes)
 {
@@ -1508,19 +1554,18 @@ int build_pyramid(b200mvs_ctx* ctx, int id, const b200mvs_undistort::Src& src, i
     for (HostLevel& L : v.lv) total += (size_t)L.pitch * L.h;
     const size_t need = pyramid_bytes(v);
     v.last_use = ++ctx->use_clock;
-    if (!v.d_base || v.bytes != need) {
+    if (v.pyr.bytes() != need) {
         // the view holds no pyramid while room is made for its new one, so it is never the one evicted for it
         drop_pyramid(ctx, v);
-        const cudaError_t e = dev_alloc(ctx, reinterpret_cast<void**>(&v.d_base), need);
+        const cudaError_t e = v.pyr.reserve(need / sizeof(uchar4));
         if (e != cudaSuccess)
             return fail(has_source(ctx) && e == cudaErrorMemoryAllocation ? B200MVS_ERR_NO_MEMORY : B200MVS_ERR_CUDA,
                         "pyramid of view %d (%zu bytes): %s", id, need, cudaGetErrorString(e));
-        v.bytes = need;
         ctx->pyr_resident += need;
     }
     size_t off = 0;
-    uint4* qbase = reinterpret_cast<uint4*>(v.d_base + total);      // total is a multiple of 4 texels: 16-byte aligned
-    for (HostLevel& L : v.lv) { L.d_img = v.d_base + off; L.d_quad = qbase + off; off += (size_t)L.pitch * L.h; }
+    uint4* qbase = reinterpret_cast<uint4*>(v.pyr.p + total);       // total is a multiple of 4 texels: 16-byte aligned
+    for (HostLevel& L : v.lv) { L.d_img = v.pyr.p + off; L.d_quad = qbase + off; off += (size_t)L.pitch * L.h; }
     const dim3 blk(32, 8);
     const dim3 grid0((v.w + 31) / 32, (v.h + 7) / 8);
     const bool planar = src.plane != 0;
@@ -1570,16 +1615,10 @@ int sync_view_params(b200mvs_ctx* ctx)
             p.lv[l].quad = v.has_image ? L.d_quad : nullptr;
         }
     }
-    CK(cudaMemcpyAsync(ctx->d_views, hp.data(), hp.size() * sizeof(ViewParams), cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_views.p, hp.data(), hp.size() * sizeof(ViewParams), cudaMemcpyHostToDevice, ctx->stream.get()));
+    CK(cudaStreamSynchronize(ctx->stream.get()));
     ctx->views_dirty = false;
     return 0;
-}
-
-cudaEvent_t get_event(b200mvs_ctx* ctx, size_t i)
-{
-    while (ctx->ev_pool.size() <= i) { cudaEvent_t e; cudaEventCreate(&e); ctx->ev_pool.push_back(e); }
-    return ctx->ev_pool[i];
 }
 
 // Opt-in to > 48 KB of dynamic shared memory and size the grids to what is resident on the chip (once per context).
@@ -1648,15 +1687,11 @@ const char* b200mvs_last_error(const b200mvs_ctx*) { return last_error.c_str(); 
 
 int b200mvs_create(int device, int n_views, b200mvs_ctx** out)
 {
-    b200mvs_ctx* ctx = nullptr;
     if (!out || n_views <= 0) return fail(B200MVS_ERR_INVALID_ARG, "b200mvs_create: bad arguments");
     *out = nullptr;
     if (device == B200MVS_DEVICE_NONE) {
         // planning context: cameras, features, global view selection (pure host logic); every compute entry point fails
-        ctx = new b200mvs_ctx();
-        ctx->device = B200MVS_DEVICE_NONE;
-        ctx->views.resize(n_views);
-        *out = ctx;
+        *out = new b200mvs_ctx(B200MVS_DEVICE_NONE, n_views);
         return 0;
     }
     int ndev = 0;
@@ -1666,19 +1701,24 @@ int b200mvs_create(int device, int n_views, b200mvs_ctx** out)
     if (device < 0 || device >= ndev) return fail(B200MVS_ERR_INVALID_ARG, "device %d out of range (%d devices)", device, ndev);
     e = cudaSetDevice(device);
     if (e != cudaSuccess) return fail(B200MVS_ERR_CUDA, "cudaSetDevice: %s", cudaGetErrorString(e));
-    ctx = new b200mvs_ctx();
-    ctx->device = device;
-    ctx->views.resize(n_views);
-    auto bail = [&](const char* what, cudaError_t ce) {
-        fail(B200MVS_ERR_CUDA, "%s: %s", what, cudaGetErrorString(ce));
-        delete ctx;
-        return B200MVS_ERR_CUDA;
-    };
-    if ((e = cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("cudaStreamCreate", e);
-    if ((e = dev_alloc(ctx, reinterpret_cast<void**>(&ctx->d_views), sizeof(ViewParams) * n_views)) != cudaSuccess) return bail("device allocation (view table)", e);
-    if ((e = dev_alloc(ctx, reinterpret_cast<void**>(&ctx->d_lut), 256 * sizeof(float))) != cudaSuccess) return bail("device allocation (sRGB table)", e);
-    if ((e = cudaMallocHost(&ctx->h_counters, sizeof(HostCounters))) != cudaSuccess) return bail("cudaMallocHost", e);
-    if ((e = cudaHostAlloc(&ctx->h_mirror, sizeof(unsigned long long) * 8192, cudaHostAllocMapped)) != cudaSuccess) return bail("cudaHostAlloc", e);
+    // on a failure the partly made context is destroyed, which frees what it holds
+    std::unique_ptr<b200mvs_ctx> ctx(new b200mvs_ctx(device, n_views));
+    auto bail = [](const char* what, cudaError_t ce) { return fail(B200MVS_ERR_CUDA, "%s: %s", what, cudaGetErrorString(ce)); };
+    cudaStream_t st = nullptr;
+    if ((e = cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking)) != cudaSuccess) return bail("cudaStreamCreate", e);
+    ctx->stream.reset(st);
+    if ((e = ctx->d_views.reserve(n_views)) != cudaSuccess) return bail("device allocation (view table)", e);
+    if ((e = ctx->d_lut.reserve(256)) != cudaSuccess) return bail("device allocation (sRGB table)", e);
+    void* h = nullptr;
+    if ((e = cudaMallocHost(&h, sizeof(HostCounters))) != cudaSuccess) return bail("cudaMallocHost", e);
+    ctx->h_counters.reset(static_cast<HostCounters*>(h));
+    if ((e = cudaHostAlloc(&h, MIRROR_BYTES, cudaHostAllocMapped)) != cudaSuccess) return bail("cudaHostAlloc", e);
+    ctx->h_mirror.reset(static_cast<HostMirror*>(h));
+    for (Event* ev : {&ctx->ev_begin, &ctx->ev_end, &ctx->ev_copied, &ctx->ev_caller, &ctx->ev_source}) {
+        cudaEvent_t made = nullptr;
+        if ((e = cudaEventCreate(&made)) != cudaSuccess) return bail("cudaEventCreate", e);
+        ev->reset(made);
+    }
     // sRGB code value -> linear: the formula documented at mvs_tools.cc:21-29; tests/test_oracle_vs_reference.py::test_srgb_table_matches_reference checks the
     // 256 floats against the reference table.
     float lut[256];
@@ -1686,30 +1726,15 @@ int b200mvs_create(int device, int n_views, b200mvs_ctx** out)
         const double x = i / 255.0;
         lut[i] = (float)((i <= 0.04045 * 255.0) ? x / 12.92 : std::pow((x + 0.055) / 1.055, 2.4));
     }
-    if ((e = cudaMemcpy(ctx->d_lut, lut, sizeof(lut), cudaMemcpyHostToDevice)) != cudaSuccess) return bail("cudaMemcpy(lut)", e);
-    *out = ctx;
+    if ((e = cudaMemcpy(ctx->d_lut.p, lut, sizeof(lut), cudaMemcpyHostToDevice)) != cudaSuccess) return bail("cudaMemcpy(lut)", e);
+    *out = ctx.release();
     return 0;
 }
 
 void b200mvs_destroy(b200mvs_ctx* ctx)
 {
     if (!ctx) return;
-    if (ctx->device == B200MVS_DEVICE_NONE) { delete ctx; return; }
-    cudaSetDevice(ctx->device);
-    for (HostView& v : ctx->views) dev_free(ctx, v.d_base, v.bytes);
-    dev_free(ctx, ctx->d_views, sizeof(ViewParams) * ctx->views.size());
-    dev_free(ctx, ctx->d_lut, 256 * sizeof(float));
-    if (ctx->h_counters) cudaFreeHost(ctx->h_counters);
-    if (ctx->h_mirror) cudaFreeHost(ctx->h_mirror);
-    for (b200mvs_ctx::Stage& S : ctx->stage) {
-        if (S.host) cudaFreeHost(S.host);
-        dev_free(ctx, S.dev, S.cap);
-        if (S.done) cudaEventDestroy(S.done);
-    }
-    release_workspace(ctx);
-    ctx->d_settings.release(ctx); ctx->ctl.release(ctx);
-    for (cudaEvent_t e : ctx->ev_pool) cudaEventDestroy(e);
-    if (ctx->stream) cudaStreamDestroy(ctx->stream);
+    if (ctx->device != B200MVS_DEVICE_NONE) cudaSetDevice(ctx->device);
     delete ctx;
 }
 
@@ -1723,20 +1748,23 @@ namespace {
 int next_stage(b200mvs_ctx* ctx, size_t bytes, bool alloc, b200mvs_ctx::Stage** out)
 {
     b200mvs_ctx::Stage& S = ctx->stage[ctx->stage_next++ & 1u];
-    if (S.busy) { CK(cudaEventSynchronize(S.done)); S.busy = false; }      // the transfer that used this slot two uploads ago
-    if (S.cap < bytes || (alloc && !S.dev)) {
-        const size_t cap = std::max(S.cap, bytes);
-        if (S.host) cudaFreeHost(S.host);
-        if (S.dev) dev_free(ctx, S.dev, S.cap);
-        else ctx->mem.resident -= S.cap;                                      // charged only
-        S.host = nullptr; S.dev = nullptr; S.cap = 0;
+    if (S.busy) { CK(cudaEventSynchronize(S.done.get())); S.busy = false; }   // the transfer that used this slot two uploads ago
+    if (S.cap() < bytes || (alloc && !S.dev.p)) {
+        // the old slot goes before the larger one is made
+        const size_t cap = std::max(S.cap(), bytes);
+        S.host.reset();
+        S.dev.release();
+        dev_uncharge(ctx, S.charged);
+        S.charged = 0;
         if (alloc) {
-            CK(cudaMallocHost(&S.host, cap));
-            CK(dev_alloc(ctx, reinterpret_cast<void**>(&S.dev), cap));
+            void* h = nullptr;
+            CK(cudaMallocHost(&h, cap));
+            S.host.reset(static_cast<uint8_t*>(h));
+            CK(S.dev.reserve(cap));
         } else {
             CK(dev_charge(ctx, cap));
+            S.charged = cap;
         }
-        S.cap = cap;
     }
     *out = &S;
     return 0;
@@ -1749,11 +1777,15 @@ int upload_host(b200mvs_ctx* ctx, int id, const uint8_t* rgb, int channels)
     const size_t bytes = (size_t)v.w * v.h * channels;
     b200mvs_ctx::Stage* S = nullptr;
     if (int rc = next_stage(ctx, bytes, true, &S)) return rc;
-    if (!S->done) CK(cudaEventCreateWithFlags(&S->done, cudaEventDisableTiming));
-    std::memcpy(S->host, rgb, bytes);                                        // pageable -> pinned; returns the caller's buffer
-    CK(cudaMemcpyAsync(S->dev, S->host, bytes, cudaMemcpyHostToDevice, ctx->stream));
-    const int rc = build_pyramid(ctx, id, b200mvs_undistort::Src{S->dev, (int64_t)v.w * channels, 0}, channels, ctx->stream);
-    CK(cudaEventRecord(S->done, ctx->stream));
+    if (!S->done) {
+        cudaEvent_t made = nullptr;
+        CK(cudaEventCreateWithFlags(&made, cudaEventDisableTiming));
+        S->done.reset(made);
+    }
+    std::memcpy(S->host.get(), rgb, bytes);                                  // pageable -> pinned; returns the caller's buffer
+    CK(cudaMemcpyAsync(S->dev.p, S->host.get(), bytes, cudaMemcpyHostToDevice, ctx->stream.get()));
+    const int rc = build_pyramid(ctx, id, b200mvs_undistort::Src{S->dev.p, (int64_t)v.w * channels, 0}, channels, ctx->stream.get());
+    CK(cudaEventRecord(S->done.get(), ctx->stream.get()));
     S->busy = true;
     // no synchronisation here: everything that reads the pyramid is ordered behind it on the context's stream
     return rc;
@@ -1792,10 +1824,9 @@ int load_device_image(b200mvs_ctx* ctx, int id, const b200mvs_device_image& im)
     if (!why.empty()) return fail(B200MVS_ERR_INVALID_ARG, "device image of view %d %s", id, why.c_str());
     b200mvs_ctx::Stage* S = nullptr;
     if (int rc = next_stage(ctx, (size_t)v.w * v.h * im.channels, false, &S)) return rc;
-    const cudaEvent_t ev = get_event(ctx, 4);
-    CK(cudaEventRecord(ev, static_cast<cudaStream_t>(im.cuda_stream)));
-    CK(cudaStreamWaitEvent(ctx->stream, ev, 0));
-    return build_pyramid(ctx, id, b200mvs_undistort::Src{im.data, im.row_pitch, im.plane_pitch}, im.channels, ctx->stream);
+    CK(cudaEventRecord(ctx->ev_source.get(), static_cast<cudaStream_t>(im.cuda_stream)));
+    CK(cudaStreamWaitEvent(ctx->stream.get(), ctx->ev_source.get(), 0));
+    return build_pyramid(ctx, id, b200mvs_undistort::Src{im.data, im.row_pitch, im.plane_pitch}, im.channels, ctx->stream.get());
 }
 
 // loadColorImage (image_pyramid.cc:56-95) for every listed view whose pyramid is not resident: through the image source on
@@ -1836,9 +1867,8 @@ int load_views(b200mvs_ctx* ctx, const std::vector<int>& ids, int* failed_view)
     }
     if (!held.empty()) {
         // one wait for every pyramid built from the caller's memory, then the images go back
-        const cudaEvent_t ev = get_event(ctx, 4);
-        cudaError_t e = cudaEventRecord(ev, ctx->stream);
-        if (e == cudaSuccess) e = cudaEventSynchronize(ev);
+        cudaError_t e = cudaEventRecord(ctx->ev_source.get(), ctx->stream.get());
+        if (e == cudaSuccess) e = cudaEventSynchronize(ctx->ev_source.get());
         if (ctx->release) for (int id : held) ctx->release(ctx->user, id);
         if (e != cudaSuccess && !rc) rc = fail(B200MVS_ERR_CUDA, "device image source: %s", cudaGetErrorString(e));
     }
@@ -1858,7 +1888,6 @@ int b200mvs_upload_view(b200mvs_ctx* ctx, int id, const uint8_t* rgb, int w, int
     if ((rc = require_device(ctx)) || (rc = check_camera_args(ctx, "b200mvs_upload_view", id, rgb != nullptr, w, h, ppoint, rot, trans))) return rc;
     if (channels < 1 || channels > 4) return fail(B200MVS_ERR_INVALID_ARG, "Image with invalid number of channels");
     CK(cudaSetDevice(ctx->device));
-    ctx->pinned.clear();
     if ((rc = set_camera(ctx, id, w, h, flen, paspect, ppoint, rot, trans))) return rc;
     return upload_host(ctx, id, rgb, channels);
 }
@@ -1873,9 +1902,8 @@ int b200mvs_upload_view_device(b200mvs_ctx* ctx, int id, const uint8_t* rgb_dev,
     if ((rc = require_device(ctx)) || (rc = check_camera_args(ctx, "b200mvs_upload_view_device", id, rgb_dev != nullptr, w, h, ppoint, rot, trans)))
         return rc;
     CK(cudaSetDevice(ctx->device));
-    ctx->pinned.clear();
     if ((rc = set_camera(ctx, id, w, h, flen, paspect, ppoint, rot, trans))) return rc;
-    cudaStream_t s = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
+    cudaStream_t s = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream.get();
     rc = build_pyramid(ctx, id, b200mvs_undistort::Src{rgb_dev, (int64_t)w * 3, 0}, 3, s);
     cudaError_t e = cudaStreamSynchronize(s);
     if (!rc && e != cudaSuccess) rc = fail(B200MVS_ERR_CUDA, "upload sync: %s", cudaGetErrorString(e));
@@ -1907,7 +1935,7 @@ int b200mvs_set_view_distortion(b200mvs_ctx* ctx, int id, float k2, float k4)
     if (v.k2 == k2 && v.k4 == k4) return 0;
     v.k2 = k2; v.k4 = k4;
     // the resident pyramid was built with the old coefficients: the view is fetched or uploaded again when needed
-    if (v.d_base) {
+    if (v.pyr.p) {
         CK(cudaSetDevice(ctx->device));
         drop_pyramid(ctx, v);
     }
@@ -1978,25 +2006,26 @@ int get_level(b200mvs_ctx* ctx, int id, int level, int* w, int* h, uint8_t* rgb,
     if (ctx->device != B200MVS_DEVICE_NONE) {
         CK(cudaSetDevice(ctx->device));
         if (rgb_dev && ((rc = check_device_buffer("b200mvs_get_level_device", "rgb_dev", rgb_dev, ctx->device, 1)) ||
-                        (rc = wait_for_stream(get_event(ctx, 3), cuda_stream, ctx->stream))))
+                        (rc = wait_for_stream(ctx->ev_caller.get(), cuda_stream, ctx->stream.get()))))
             return rc;
     }
+    const PinsOfCall pins(ctx);
     pin_views(ctx, {id});
     if ((rc = load_views(ctx, {id}, nullptr))) return rc;   // an evicted view is fetched again through the source
     const dim3 grid((L.w + 31) / 32, (L.h + 7) / 8), blk(32, 8);
+    const cudaStream_t st = ctx->stream.get();
     if (rgb_dev) {
-        k_export_rgb<<<grid, blk, 0, ctx->stream>>>(L.d_img, L.w, L.h, L.pitch, rgb_dev);
+        k_export_rgb<<<grid, blk, 0, st>>>(L.d_img, L.w, L.h, L.pitch, rgb_dev);
         CK(cudaGetLastError());
-        CK(cudaStreamSynchronize(ctx->stream));
+        CK(cudaStreamSynchronize(st));
         return 0;
     }
-    uint8_t* d = nullptr;
+    DevBuf<uint8_t> d(ctx);
     const size_t bytes = (size_t)L.w * L.h * 3;
-    CK(dev_alloc(ctx, reinterpret_cast<void**>(&d), bytes));
-    k_export_rgb<<<grid, blk, 0, ctx->stream>>>(L.d_img, L.w, L.h, L.pitch, d);
-    cudaError_t e = cudaMemcpyAsync(rgb, d, bytes, cudaMemcpyDeviceToHost, ctx->stream);
-    cudaStreamSynchronize(ctx->stream);
-    dev_free(ctx, d, bytes);
+    CK(d.reserve(bytes));
+    k_export_rgb<<<grid, blk, 0, st>>>(L.d_img, L.w, L.h, L.pitch, d.p);
+    cudaError_t e = cudaMemcpyAsync(rgb, d.p, bytes, cudaMemcpyDeviceToHost, st);
+    cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail(B200MVS_ERR_CUDA, "get_level copy: %s", cudaGetErrorString(e));
     return 0;
 }
@@ -2105,6 +2134,7 @@ int b200mvs_optimize_patches(b200mvs_ctx* ctx, const b200mvs_settings* s, int re
     CK(cudaSetDevice(ctx->device));
     std::vector<int> need(gsel);
     need.push_back(ref);
+    const PinsOfCall pins(ctx);
     pin_views(ctx, need);
     if ((rc = load_views(ctx, need, nullptr))) return rc;
     if (stats) std::memset(stats, 0, sizeof(*stats));
@@ -2126,18 +2156,18 @@ int b200mvs_optimize_patches(b200mvs_ctx* ctx, const b200mvs_settings* s, int re
     if (ctx->mem.resident + (uint64_t)n * (sizeof(Entry) + sizeof(PatchOut)) + sizeof(JobParams) + 4096 > budget_limit(ctx))
         release_workspace(ctx);
     WorkspaceInUse in_use(ctx);
-    CK(ctx->run_in.reserve(ctx, n));
-    CK(ctx->run_out.reserve(ctx, n));
-    CK(ctx->counters.reserve(ctx, C_NUM + 8));
-    CK(ctx->d_jobs.reserve(ctx, 1));
-    CK(ctx->d_settings.reserve(ctx, 1));
+    CK(ctx->run_in.reserve(n));
+    CK(ctx->run_out.reserve(n));
+    CK(ctx->counters.reserve(C_NUM + 8));
+    CK(ctx->d_jobs.reserve(1));
+    CK(ctx->d_settings.reserve(1));
     const DevSettings ds = to_dev(*s);
-    cudaStream_t st = ctx->stream;
+    cudaStream_t st = ctx->stream.get();
     CK(cudaMemcpyAsync(ctx->run_in.p, he.data(), sizeof(Entry) * n, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(ctx->d_jobs.p, &J, sizeof(J), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(ctx->d_settings.p, &ds, sizeof(ds), cudaMemcpyHostToDevice, st));
     CK(cudaMemsetAsync(ctx->counters.p, 0, sizeof(unsigned long long) * C_NUM, st));
-    cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1);
+    cudaEvent_t e0 = ctx->ev_begin.get(), e1 = ctx->ev_end.get();
     CK(cudaEventRecord(e0, st));
     {
         int rc2 = prepare_kernels(ctx);
@@ -2145,7 +2175,7 @@ int b200mvs_optimize_patches(b200mvs_ctx* ctx, const b200mvs_settings* s, int re
         const int warps_per_block = OPT_TPB / 32;
         const int grid = std::max(1, std::min((n + warps_per_block - 1) / warps_per_block, ctx->optimize_grid));
         k_optimize<<<grid, OPT_TPB, OPT_SMEM_BYTES, st>>>(ctx->run_in.p, ctx->run_out.p, n, ctx->optimize_mode, ctx->d_settings.p,
-                                                          ctx->d_jobs.p, ctx->d_views, ctx->d_lut, ctx->counters.p);
+                                                          ctx->d_jobs.p, ctx->d_views.p, ctx->d_lut.p, ctx->counters.p);
     }
     CK(cudaGetLastError());
     CK(cudaEventRecord(e1, st));
@@ -2211,21 +2241,6 @@ __global__ void __launch_bounds__(PLAN_TPB) k_plan_views(const b200mvs_plan::Pla
     B.bind(&in, &jobs[blockIdx.x], ws, out);
     b200mvs_plan::plan_view(B, (int)threadIdx.x, (int)blockDim.x, BlockSync{});
 }
-
-// Device allocations of one planning call, freed when it ends
-struct PlanAllocs {
-    b200mvs_ctx* ctx;
-    std::vector<std::pair<void*, size_t>> held;
-    explicit PlanAllocs(b200mvs_ctx* c) : ctx(c) {}
-    ~PlanAllocs() { while (!held.empty()) pop(); }
-    cudaError_t push(size_t bytes, void** p)
-    {
-        const cudaError_t e = dev_alloc(ctx, p, bytes);
-        if (e == cudaSuccess) held.emplace_back(*p, bytes);
-        return e;
-    }
-    void pop() { dev_free(ctx, held.back().first, held.back().second); held.pop_back(); }
-};
 
 inline size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 
@@ -2306,17 +2321,16 @@ int plan_on_device(b200mvs_ctx* ctx, const b200mvs_settings& s, const int32_t* r
     }
     if (in_bytes >= avail) return 0;
     avail -= in_bytes;
-    PlanAllocs A(ctx);
-    void* d_in = nullptr;
-    CK(A.push(in_bytes, &d_in));
-    cudaStream_t st = ctx->stream;
+    DevBuf<char> d_in(ctx);
+    CK(d_in.reserve(in_bytes));
+    cudaStream_t st = ctx->stream.get();
     PL::PlanInput in = {};
     {
         const void* dptr[7];
         size_t o = 0;
         for (int k = 0; k < 7; ++k) {
-            dptr[k] = static_cast<char*>(d_in) + o;
-            if (parts[k].second) CK(cudaMemcpyAsync(static_cast<char*>(d_in) + o, parts[k].first, parts[k].second, cudaMemcpyHostToDevice, st));
+            dptr[k] = d_in.p + o;
+            if (parts[k].second) CK(cudaMemcpyAsync(d_in.p + o, parts[k].first, parts[k].second, cudaMemcpyHostToDevice, st));
             o += align256(parts[k].second);
         }
         in.views = static_cast<const PL::PlanView*>(dptr[0]);
@@ -2344,16 +2358,17 @@ int plan_on_device(b200mvs_ctx* ctx, const b200mvs_settings& s, const int32_t* r
             hj[k].out = out_words; out_words += PL::out_words(hj[k].seed_cap);
         }
         const size_t jobs_bytes = align256(n * sizeof(PL::PlanJob));
-        void* d_ws = nullptr; void* d_out = nullptr;
-        CK(A.push(align256(ws_words * 4), &d_ws));
-        CK(A.push(jobs_bytes + out_words * 4, &d_out));
+        // the chunk's workspace and results, freed in reverse order before the next chunk
+        DevBuf<char> d_ws(ctx), d_out(ctx);
+        CK(d_ws.reserve(align256(ws_words * 4)));
+        CK(d_out.reserve(jobs_bytes + out_words * 4));
         info.peak_bytes = std::max<uint64_t>(info.peak_bytes, in_bytes + align256(ws_words * 4) + jobs_bytes + out_words * 4);
-        uint32_t* d_res = reinterpret_cast<uint32_t*>(static_cast<char*>(d_out) + jobs_bytes);
-        CK(cudaMemcpyAsync(d_out, hj.data(), n * sizeof(PL::PlanJob), cudaMemcpyHostToDevice, st));
+        uint32_t* d_res = reinterpret_cast<uint32_t*>(d_out.p + jobs_bytes);
+        CK(cudaMemcpyAsync(d_out.p, hj.data(), n * sizeof(PL::PlanJob), cudaMemcpyHostToDevice, st));
         CK(cudaMemsetAsync(d_res, 0, out_words * 4, st));
-        cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1);
+        cudaEvent_t e0 = ctx->ev_begin.get(), e1 = ctx->ev_end.get();
         CK(cudaEventRecord(e0, st));
-        k_plan_views<<<(unsigned)n, PLAN_TPB, 0, st>>>(in, static_cast<const PL::PlanJob*>(d_out), static_cast<uint32_t*>(d_ws), d_res);
+        k_plan_views<<<(unsigned)n, PLAN_TPB, 0, st>>>(in, reinterpret_cast<const PL::PlanJob*>(d_out.p), reinterpret_cast<uint32_t*>(d_ws.p), d_res);
         CK(cudaGetLastError());
         CK(cudaEventRecord(e1, st));
         std::vector<uint32_t> res(out_words);
@@ -2362,7 +2377,6 @@ int plan_on_device(b200mvs_ctx* ctx, const b200mvs_settings& s, const int32_t* r
         float ms = 0.f;
         CK(cudaEventElapsedTime(&ms, e0, e1));
         info.ms_device += ms;
-        A.pop(); A.pop();
         for (size_t k = 0; k < n; ++k) {
             const uint32_t* r = &res[hj[k].out];
             const int j = jobs[k0 + k].j;
@@ -2522,15 +2536,15 @@ int grow_frontier(b200mvs_ctx* ctx, const FrontierCtl& c, FrontierParams& P, siz
     DevBuf<Entry>& live_run = c.resume_sorted ? ctx->run_sorted : ctx->run_in;
     DevBuf<Entry>& dead_run = c.resume_sorted ? ctx->run_in : ctx->run_sorted;
     const size_t n_run = (size_t)c.resume_nrun, carried = (size_t)c.nlist[1 - p];
-    cudaStream_t st = ctx->stream;
-    if (dead_list.cap < n) dead_list.release(ctx);
-    if (dead_run.cap < n) dead_run.release(ctx);
-    cudaError_t e = ctx->written.grow(ctx, n, n_run, st);
-    if (e == cudaSuccess) e = ctx->run_out.grow(ctx, n, n_run, st);
-    if (e == cudaSuccess) e = live_list.grow(ctx, n, carried, st);
-    if (e == cudaSuccess) e = live_run.grow(ctx, n, n_run, st);
-    if (e == cudaSuccess) e = dead_list.reserve(ctx, n);
-    if (e == cudaSuccess) e = dead_run.reserve(ctx, n);
+    cudaStream_t st = ctx->stream.get();
+    if (dead_list.cap < n) dead_list.release();
+    if (dead_run.cap < n) dead_run.release();
+    cudaError_t e = ctx->written.grow(n, n_run, st);
+    if (e == cudaSuccess) e = ctx->run_out.grow(n, n_run, st);
+    if (e == cudaSuccess) e = live_list.grow(n, carried, st);
+    if (e == cudaSuccess) e = live_run.grow(n, n_run, st);
+    if (e == cudaSuccess) e = dead_list.reserve(n);
+    if (e == cudaSuccess) e = dead_run.reserve(n);
     if (e != cudaSuccess)
         return fail(B200MVS_ERR_OVERFLOW, "frontier overflow: the next round needs %llu entries, growing to %llu failed: %s",
                     (unsigned long long)need, (unsigned long long)n, cudaGetErrorString(e));
@@ -2567,8 +2581,8 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
     }
     int rc = 0;
     const int n_refs = (int)js.size();
-    cudaStream_t st = ctx->stream;
-    std::memset(ctx->h_counters, 0, sizeof(HostCounters));
+    cudaStream_t st = ctx->stream.get();
+    std::memset(ctx->h_counters.get(), 0, sizeof(HostCounters));
     Workspace W(*s, ctx->frontier_cap);
     for (int j : js) W.add(view_workspace(ctx, *s, refs[j], plans[j].seeds.size()));
     WorkspaceInUse in_use(ctx);
@@ -2621,7 +2635,7 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
     // ---- device buffers: the sizes of b200mvs_working_set ----
     {
         cudaError_t e = cudaSuccess;
-        for_each_workspace(ctx, W, [&](auto& buf, size_t n) { if (e == cudaSuccess) e = buf.reserve(ctx, n); });
+        for_each_workspace(ctx, W, [&](auto& buf, size_t n) { if (e == cudaSuccess) e = buf.reserve(n); });
         if (e != cudaSuccess)
             return fail(B200MVS_ERR_CUDA, "workspace of %llu bytes for %d reference views: %s",
                         (unsigned long long)workspace_bytes(ctx, W), n_refs, cudaGetErrorString(e));
@@ -2666,8 +2680,8 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
     size_t cap = W.cap();
     const bool thresholded = W.thresholded;
     CK(cudaMemsetAsync(ctx->tile_cnt.p, 0, sizeof(unsigned) * n_tiles, st));
-    CK(ctx->d_settings.reserve(ctx, 1));
-    CK(ctx->ctl.reserve(ctx, 1));
+    CK(ctx->d_settings.reserve(1));
+    CK(ctx->ctl.reserve(1));
     CK(cudaMemsetAsync(ctx->job_run.p, 0, sizeof(unsigned long long) * n_refs, st));
     const DevSettings ds = to_dev(*s);
     CK(cudaMemcpyAsync(ctx->d_jobs.p, jobs.data(), sizeof(JobParams) * n_refs, cudaMemcpyHostToDevice, st));
@@ -2676,8 +2690,8 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
     CK(cudaMemsetAsync(ctx->ctl.p, 0, sizeof(FrontierCtl), st));
     if (thresholded) CK(cudaMemsetAsync(ctx->hist.p, 0, sizeof(unsigned) * (size_t)n_refs * HIST_PER_JOB, st));
     if (!seeds.empty()) CK(cudaMemcpyAsync(ctx->run_in.p, seeds.data(), sizeof(Entry) * seeds.size(), cudaMemcpyHostToDevice, st));
-    HostMirror* mirror = reinterpret_cast<HostMirror*>(ctx->h_mirror);
-    std::memset(ctx->h_mirror, 0, sizeof(HostMirror) + (sizeof(unsigned long long) + sizeof(int)) * n_refs);
+    HostMirror* mirror = ctx->h_mirror.get();
+    std::memset(mirror, 0, sizeof(HostMirror) + (sizeof(unsigned long long) + sizeof(int)) * n_refs);
     volatile unsigned long long* m_filled = reinterpret_cast<volatile unsigned long long*>(mirror + 1);
     volatile int* m_cancel_job = reinterpret_cast<volatile int*>(m_filled + n_refs);
     CK(cudaMemsetAsync(ctx->job_cancel.p, 0, sizeof(int) * n_refs, st));
@@ -2688,7 +2702,7 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
     P.run2 = ctx->run_sorted.p; P.tile_cnt = ctx->tile_cnt.p; P.tile_off = ctx->tile_off.p;
     P.n_tiles = (long long)n_tiles;
     P.cap = cap; P.n_seeds = (int)seeds.size(); P.n_jobs = n_refs;
-    P.st = ctx->d_settings.p; P.jobs = ctx->d_jobs.p; P.views = ctx->d_views; P.lut = ctx->d_lut;
+    P.st = ctx->d_settings.p; P.jobs = ctx->d_jobs.p; P.views = ctx->d_views.p; P.lut = ctx->d_lut.p;
     P.counters = ctx->counters.p; P.ctl = ctx->ctl.p; P.hist = ctx->hist.p; P.thr_bin = ctx->thr_bin.p;
     P.host = mirror; P.host_filled = m_filled; P.host_cancel_job = m_cancel_job; P.job_cancel = ctx->job_cancel.p; P.job_run = ctx->job_run.p;
     P.thread_min = ctx->thread_min >= 0 ? ctx->thread_min : OPT_THREAD_MIN;
@@ -2707,7 +2721,7 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
     float ms_all = 0.f;
     uint64_t n_launches = 0, n_resumes = 0;
     for (;;) {
-        cudaEvent_t ev_begin = get_event(ctx, 0), ev_end = get_event(ctx, 1);
+        cudaEvent_t ev_begin = ctx->ev_begin.get(), ev_end = ctx->ev_end.get();
         CK(cudaEventRecord(ev_begin, st));
         {
             void* args[] = {(void*)&P};
@@ -2721,7 +2735,7 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
         CK(cudaEventRecord(ev_end, st));
         CK(cudaMemcpyAsync(ctx->h_counters->count, ctx->counters.p, sizeof(unsigned long long) * (C_NUM + n_refs), cudaMemcpyDeviceToHost, st));
         CK(cudaMemcpyAsync(h_ctl, ctx->ctl.p, sizeof(FrontierCtl), cudaMemcpyDeviceToHost, st));
-        cudaEvent_t ev_copied = get_event(ctx, 2);
+        cudaEvent_t ev_copied = ctx->ev_copied.get();
         CK(cudaEventRecord(ev_copied, st));
         // While the kernel runs the host only relays: progress out (Progress::filled / queueSize, fancy_progress_printer.cc:84-91)
         // and cancel requests in (imageoperations.cc:177-184): a cancelled view's queue is dropped at the next round, the other
@@ -2820,6 +2834,7 @@ int reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const i
     if (stats) std::memset(stats, 0, sizeof(*stats));
     ctx->fr_initial = ctx->fr_final = ctx->fr_resumes = 0;
     ctx->plan_info = b200mvs_plan_info{};
+    const PinsOfCall pins(ctx);                  // each group pins the views it needs (run_group)
     std::vector<HostPlan> plans;
     int rc = plan_batch(ctx, s, n_refs, refs, true, true, progress, failed_view, plans);
     if (rc) return rc;
@@ -2858,7 +2873,6 @@ int reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const i
         for (int j = 0; j < n_refs; ++j) if (group_of[j] == g) js.push_back(j);
         if ((rc = run_group(ctx, s, js, refs, plans, sink, reserve, progress, stats, failed_view, view_cancelled))) return rc;
     }
-    ctx->pinned.clear();
     if (std::all_of(view_cancelled.begin(), view_cancelled.end(), [](char c) { return c != 0; }))
         return fail(B200MVS_ERR_CANCELLED, "reconstruction cancelled");
     return 0;
@@ -2874,7 +2888,7 @@ MapSink buffer_sink(b200mvs_ctx* ctx, b200mvs_maps* maps, bool on_device)
     sink.take = [ctx, maps, on_device, hslots = std::vector<unsigned>()](int j, const JobParams& J) mutable {
         const b200mvs_maps& m = maps[j];
         const size_t np = (size_t)J.W * J.H;
-        const cudaStream_t st = ctx->stream;
+        const cudaStream_t st = ctx->stream.get();
         const cudaMemcpyKind kind = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
         if (m.depth) CK(cudaMemcpyAsync(m.depth, J.depth, np * 4, kind, st));
         if (m.conf) CK(cudaMemcpyAsync(m.conf, J.conf, np * 4, kind, st));
@@ -2930,7 +2944,7 @@ int b200mvs_reconstruct_device(b200mvs_ctx* ctx, const b200mvs_settings* s, int 
         for (const auto& b : bufs)
             if (b.first && (rc = check_device_buffer(fn, what(b.second), b.first, ctx->device, 4))) return rc;
     }
-    if ((rc = wait_for_stream(get_event(ctx, 3), cuda_stream, ctx->stream))) return rc;
+    if ((rc = wait_for_stream(ctx->ev_caller.get(), cuda_stream, ctx->stream.get()))) return rc;
     const MapSink sink = buffer_sink(ctx, maps_dev, true);
     return reconstruct(ctx, s, n_refs, refs, &sink, progress, stats, failed_view);
 }
@@ -2962,9 +2976,16 @@ int b200mvs_pset_add_reconstruction(b200mvs_pset* ps, b200mvs_ctx* ctx, const b2
         const int rc = PD::extract(ps, refs[j], J.depth, J.W, J.H, L.d_img, L.pitch, cam, blocks[j]);
         return rc ? fail(rc, "view %d: %s", refs[j], last_error.c_str()) : 0;
     };
-    PD::use_allocator(ps, &A);
-    const int rc = reconstruct(ctx, s, n_refs, refs, &sink, progress, stats, failed_view);
-    PD::use_allocator(ps, nullptr);
+    struct UsingAllocator {
+        b200mvs_pset* ps;
+        UsingAllocator(b200mvs_pset* p, const PD::Allocator* a) : ps(p) { PD::use_allocator(ps, a); }
+        ~UsingAllocator() { PD::use_allocator(ps, nullptr); }
+    };
+    int rc;
+    {
+        const UsingAllocator using_ctx(ps, &A);
+        rc = reconstruct(ctx, s, n_refs, refs, &sink, progress, stats, failed_view);
+    }
     if (rc) { PD::discard(ps); return rc; }
     return PD::commit(ps, blocks, views_out);
 }
@@ -2992,7 +3013,6 @@ int set_source(b200mvs_ctx* ctx, b200mvs_fetch_fn fetch, b200mvs_device_fetch_fn
     }
     ctx->fetch = fetch; ctx->fetch_device = fetch_device; ctx->release = release; ctx->user = user;
     ctx->mem.budget = budget_bytes;
-    ctx->pinned.clear();
     make_room(ctx, 0);                 // idle workspace and then pyramids go until the resident bytes fit
     ctx->mem.peak = ctx->mem.resident;
     return 0;

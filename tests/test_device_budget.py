@@ -132,19 +132,51 @@ def test_plan_batches_prefers_shared_pyramids():
     assert second in members
 
 
-def test_cuda_malloc_only_in_the_accounted_allocator():
+def _source():
     src = open(os.path.join(ROOT, "mve_b200", "csrc", "b200mvs.cu")).read()
     src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-    src = re.sub(r"//[^\n]*", "", src)
-    spans = []
-    for head in (r"cudaError_t dev_alloc\([^)]*\)\s*\{", r"void dev_free\([^)]*\)\s*\{"):
-        m = re.search(head, src)
-        assert m, head
-        depth, i = 1, m.end()
-        while depth:
-            depth += {"{": 1, "}": -1}.get(src[i], 0)
-            i += 1
-        spans.append((m.start(), i))
-    calls = [m.start() for m in re.finditer(r"\bcuda(Malloc|Free)\s*\(", src)]
+    return re.sub(r"//[^\n]*", "", src)
+
+
+def _span(src, head):
+    """Where the definition that starts with `head` (a pattern ending at its opening brace) begins and ends."""
+    m = re.search(head, src)
+    assert m, head
+    depth, i = 1, m.end()
+    while depth:
+        depth += {"{": 1, "}": -1}.get(src[i], 0)
+        i += 1
+    return m.start(), i
+
+
+def _only_in(src, call, heads):
+    """The positions of `call`, after checking that there is one and that each lies in one of the definitions `heads`."""
+    spans = [_span(src, h) for h in heads]
+    calls = [m.start() for m in re.finditer(call, src)]
+    assert calls, call
+    assert all(any(a <= c < b for a, b in spans) for c in calls), call
+    return calls
+
+
+def test_cuda_malloc_only_in_the_accounted_allocator():
+    src = _source()
+    calls = _only_in(src, r"\bcuda(Malloc|Free)\s*\(", (r"cudaError_t dev_alloc\([^)]*\)\s*\{", r"void dev_free\([^)]*\)\s*\{"))
     assert len(calls) == 2
-    assert all(any(a <= c < b for a, b in spans) for c in calls)
+
+
+def test_context_resources_have_one_owner():
+    """Pinned blocks, events and the stream are made only where their owner is (the context, a staging slot) and freed
+    only by the owners' deleters; b200mvs_destroy frees nothing by hand, and only the accounted allocator changes the
+    resident bytes."""
+    src = _source()
+    create, destroy = r"int b200mvs_create\([^)]*\)\s*\{", r"void b200mvs_destroy\([^)]*\)\s*\{"
+    stage = (r"int next_stage\([^)]*\)\s*\{", r"int upload_host\([^)]*\)\s*\{")
+    _only_in(src, r"\bcuda(MallocHost|HostAlloc|FreeHost)\s*\(", (create, *stage, r"struct FreeHost\s*\{"))
+    _only_in(src, r"\bcudaEvent(Create\w*|Destroy)\s*\(", (create, *stage, r"struct DestroyEvent\s*\{"))
+    _only_in(src, r"\bcudaStream(Create\w*|Destroy)\s*\(", (create, r"struct DestroyStream\s*\{"))
+    a, b = _span(src, destroy)
+    assert not re.search(r"\b(cuda\w*(Free\w*|Destroy)|dev_free|release\w*)\s*\(", src[a:b]), src[a:b]
+    _only_in(src, r"\bmem\.resident\s*[-+]?=(?!=)", [r"%s\([^)]*\)\s*\{" % f for f in
+                                                      ("cudaError_t dev_alloc", "cudaError_t dev_charge", "void dev_uncharge", "void dev_free")])
+    for gone in ("ev_pool", "get_event", "PlanAllocs", "pinned.clear()"):
+        assert gone not in src, gone

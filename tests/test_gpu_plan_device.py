@@ -108,6 +108,18 @@ def _many_refs(s, times):
     return [np.repeat(np.sort(np.asarray(r, np.int32)), times) for r in s.feat_refs]
 
 
+def _lazy(s, budget, many, fetch=None):
+    """Scene `s` with the features `many` and a small frontier workspace, its images loaded on demand within `budget`
+    (through `fetch` when given)."""
+    from mve_b200 import dmrecon
+    sc = dmrecon.Scene.from_synth(s, lazy=True, budget_bytes=budget)
+    if fetch is not None:
+        sc.set_image_source(fetch, budget)
+    sc.set_features(s.feat_pos, many)
+    sc.set_frontier_capacity(0.25, 4096)          # maps do not depend on it
+    return sc
+
+
 def test_budget_groups_chunks_and_host_fallback():
     """Under a budget: groups out of ref order, planning chunks of one view, and views whose planning workspace does not
     fit on its own planned on host threads; the maps equal those of the whole batch in one call, and the peak stays
@@ -133,9 +145,7 @@ def test_budget_groups_chunks_and_host_fallback():
     if single_ws < single_plan - (1 << 20):
         budgets["host"] = fixed + single_ws
     for tag, budget in budgets.items():
-        sc = dmrecon.Scene.from_synth(s, lazy=True, budget_bytes=budget)
-        sc.set_features(s.feat_pos, many)
-        sc.set_frontier_capacity(0.25, 4096)
+        sc = _lazy(s, budget, many)
         got, gst = sc.reconstruct(st, refs)
         info = sc.plan_info()
         mem = sc.memory_stats()
@@ -150,6 +160,69 @@ def test_budget_groups_chunks_and_host_fallback():
         _same_counters(wst, gst, [k for k in COUNTERS if k != "n_rounds"])   # rounds add up over groups
         sc.close()
     assert "host" in budgets, (single_ws, single_plan)
+
+
+@pytest.mark.parametrize("before", ["level", "optimize_patches", "failed_reconstruction"])
+def test_pins_last_one_call(before):
+    """The views a call pins are unpinned when it returns, also after a level read, a patch optimisation and a failed
+    reconstruction.  The budget fits the planning workspace of the next reconstruction only when a resident pyramid is
+    evicted, so it plans as on a context that skipped the earlier call: every view on the device, with the same maps."""
+    from mve_b200 import dmrecon
+    s = golden_scene("T2")
+    refs = list(range(s.n_views))[::-1]
+    st = _settings(s)
+    many = _many_refs(s, 512)
+    whole = dmrecon.Scene.from_synth(s)
+    whole.set_features(s.feat_pos, many)
+    whole.set_frontier_capacity(0.25, 4096)
+    single_plan = max(0, *[(whole.reconstruct(st, [r]), whole.plan_info()["peak_bytes"])[1] for r in refs])
+    fixed = whole.memory_stats().fixed
+    single_ws = max(whole.working_set(st, [r]) for r in refs)
+    whole.close()
+    assert single_ws < single_plan, (single_ws, single_plan)
+    budget = fixed + single_plan + 4096
+
+    def routes(sc):
+        maps, stats = sc.reconstruct(st, refs)
+        info = sc.plan_info()
+        return maps, stats, (info["n_prepared"], info["n_device"], info["n_host"])
+
+    sc = _lazy(s, budget, many)
+    want, wst, want_routes = routes(sc)
+    sc.close()
+    assert want_routes == (0, len(refs), 0), want_routes
+    failing = {"view": -1}
+
+    def fetch(view):
+        if view == failing["view"]:
+            raise RuntimeError("view %d is not available" % view)
+        return s.images[view]
+
+    sc = _lazy(s, budget, many, fetch)
+    v = 0
+    if before == "level":
+        sc.level(v, 0)
+    elif before == "optimize_patches":
+        m = want[refs.index(v)]
+        y, x = np.nonzero(m["conf"] > 0)
+        y, x = y[:64], x[:64]
+        pin = np.zeros(len(y), dmrecon.PATCH_IN)
+        pin["x"], pin["y"], pin["depth"] = x, y, m["depth"][y, x]
+        pin["dz_i"], pin["dz_j"] = m["dz"][y, x, 0], m["dz"][y, x, 1]
+        pin["n_local"] = 4
+        pin["local_ids"] = m["view_ids"][y, x]
+        assert (sc.optimize_patches(st, v, sc.global_view_selection(st, v), pin)["conf"] > 0).any()
+    else:
+        failing["view"] = refs[0]                   # the first group's reference view, loaded after its neighbours
+        with pytest.raises(dmrecon.B200MVSError):
+            sc.reconstruct(st, refs)
+        failing["view"] = -1
+    got, gst, got_routes = routes(sc)
+    assert got_routes == want_routes, got_routes
+    _same_maps(want, got)
+    _same_counters(wst, gst, [k for k in COUNTERS if k != "n_rounds"])   # rounds add up over groups
+    assert sc.memory_stats().peak <= budget
+    sc.close()
 
 
 def test_empty_selection_fails_the_same_way():
