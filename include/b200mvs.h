@@ -398,12 +398,37 @@ int b200mvs_plan_batches(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs
                          uint64_t available, int32_t* group_of_ref, int32_t* failed_view_or_null);
 
 /* ---- consumers of the depth maps, on the device (SURVEY.md 8f rank 2 and 3).  Stateless: host buffers in, host buffers
- *      out, `device` = CUDA device ordinal.  Errors: negative code, message from b200mvs_last_error(). ---- */
+ *      out (the *_device forms: device buffers in and out), `device` = CUDA device ordinal.  Errors: negative code, message
+ *      from b200mvs_last_error(). ---- */
 const char* b200mvs_depthmap_last_error(void);   /* the same message as b200mvs_last_error */
 /* mve::image::depthmap_confidence_clean (libs/mve/depthmap.cc:118-131): depth = 0 where conf <= 0, in place. */
 int b200mvs_depthmap_confidence_clean(int device, float* depth, const float* conf, int w, int h);
 /* mve::image::depthmap_cleanup (depthmap.cc:25-113): 4-connected islands of depth != 0 smaller than thres pixels are erased. */
 int b200mvs_depthmap_cleanup(int device, const float* depth, int w, int h, int64_t thres, float* out);
+/* The two filters above on n_maps maps of their own sizes (widths[j] x heights[j]) in DEVICE memory on `device`, for GPU
+ * callers that hold the maps of b200mvs_reconstruct_device:
+ *   - Results: every output map is byte for byte what the host entry point gives for the same map (and threshold),
+ *     NaN, +-inf and -0.0 depths and confidences included; a negative threshold is converted to size_t as the reference
+ *     does, which erases every island.
+ *   - Checks, all before anything is launched or written; a failure is B200MVS_ERR_INVALID_ARG with a message naming the
+ *     function, the map index and the field: n_maps < 0; a NULL array, or a NULL map, when n_maps > 0; a width or height
+ *     < 1; a map of more than 0xFFFFFFF0 pixels (the host entry point's limit); a buffer that is host memory (pageable or
+ *     pinned), memory of another device or not 4-byte aligned (cudaPointerGetAttributes, as b200mvs_reconstruct_device
+ *     checks its maps); a written range (depth_dev of confidence_clean, out_dev of cleanup) that overlaps any other range
+ *     of the call, except out_dev[j] == depth_dev[j].  n_maps == 0 returns 0 and touches nothing.
+ *   - Streams: the work runs on cuda_stream (a cudaStream_t; NULL = the legacy default stream) after what is already
+ *     there, and the call returns when the maps are written.
+ *   - Memory: the maps are read and written in place in the caller's buffers, with no staging copy.  cleanup takes its
+ *     maps in order in chunks, each the longest run of consecutive maps of at most 2^28 pixels in all (a larger map is a
+ *     chunk of its own), and allocates once per call a union-find workspace of 8 B per pixel of the largest chunk; both
+ *     also hold a table of 56 B per map and 4 B per 256 pixels of a map.  Everything is freed before the call returns. */
+/* depthmap_confidence_clean on each map: depth_dev[j] = 0 where conf_dev[j] <= 0, in place. */
+int b200mvs_depthmap_confidence_clean_device(int device, int n_maps, float* const* depth_dev, const float* const* conf_dev,
+                                             const int32_t* widths, const int32_t* heights, void* cuda_stream);
+/* depthmap_cleanup on each map: out_dev[j] = depth_dev[j] with the 4-connected islands of depth != 0 smaller than thres[j]
+ * pixels erased.  out_dev[j] == depth_dev[j] cleans in place. */
+int b200mvs_depthmap_cleanup_device(int device, int n_maps, const float* const* depth_dev, const int32_t* widths,
+                                    const int32_t* heights, const int64_t* thres, float* const* out_dev, void* cuda_stream);
 /* mve::geom::depthmap_triangulate (depthmap.cc:196-375, the per-view work of apps/scene2pset/scene2pset.cc:264-328):
  * vertex ids per pixel (0xFFFFFFFF = none), vertices (pixel_3dpos; transformed by the 4x4 row-major cam_to_world when given,
  * like mesh_transform), vertex colours (r, g, b, 1 as floats; NULL colour image = none) and faces, all in the reference's
