@@ -2,10 +2,13 @@
 analyzeFeatures + GlobalViewSelection (dmrecon.cc:179-241, global_view_selection.cc) - restructured for speed in
 mve_b200/csrc/b200mvs.cu - and must reproduce the reference's printed selections exactly (golden lines from
 oracle/_ref/dmrecon, tests/golden/make_golden.py); compute entry points must refuse to run."""
+import os
+import re
+
 import numpy as np
 import pytest
 
-from tests.util import golden_ref, golden_scene
+from tests.util import ROOT, golden_ref, golden_scene
 
 
 def _planning_scene(s, n_views=None):
@@ -131,3 +134,19 @@ def test_planned_selection_is_what_global_view_selection_returns(monkeypatch):
         for v in range(s.n_views):
             assert g.global_view_selection(st, v) == ref["gvs_default_%d" % v].tolist(), (threads, v)       # looked up
             assert g.global_view_selection(st3, v) == ref["gvs_n3_%d" % v].tolist(), (threads, v)           # other settings: computed
+
+
+def test_planning_arithmetic_is_written_once():
+    """The host planner calls the planning helpers of plan_device.cuh, the ones the device planner calls, and reads the
+    features in the arrays both planners share: b200mvs.cu defines no copy of a helper, no feature record of its own and
+    no second seed type."""
+    src = open(os.path.join(ROOT, "mve_b200", "csrc", "b200mvs.cu")).read()
+    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
+    src = re.sub(r"//[^\n]*", "", src)
+    helpers = ("fadd", "fmul", "fdiv", "fsqrt", "ddiv", "ffloor", "fceil", "dot3", "world_to_cam", "mat3_mul",
+               "point_in_frustum", "in_aabb", "unit_dir", "foot_print", "round_mve", "seen_in_box", "footprint_ratio",
+               "seed_of")
+    for name in helpers:
+        assert not re.search(r"\b(float|double|bool|void|auto)\s+%s\s*[(=]" % name, src), name
+    for gone in ("HostFeature", "SeedPoint"):
+        assert not re.search(r"\b%s\b" % gone, src), gone
