@@ -451,6 +451,55 @@ int b200mvs_depthmap_pointset(int device, const float* depth, int w, int h, cons
                               uint64_t cap_vertices, uint64_t cap_faces, uint64_t* n_vertices, uint64_t* n_faces,
                               double* device_ms_or_null);
 
+/* b200mvs_depthmap_pointset (and with the attribute outputs NULL, b200mvs_depthmap_triangulate) on n_maps maps of their
+ * own sizes in DEVICE memory on `device`, for GPU callers that hold the maps and level images of
+ * b200mvs_reconstruct_device.  One b200mvs_dm_mesh per map: its inputs, its outputs and, on return, its counts.
+ *   - Results: each map's outputs are byte for byte what b200mvs_depthmap_pointset gives for that map alone with the same
+ *     invproj, cam_to_world, colour image, dd_factor, conf_iterations and scale_factor: vertex ids (0xFFFFFFFF = none),
+ *     vertex and face order, and every float, NaN, +-inf and -0.0 depths included.  Vertex ids and face indices start at
+ *     0 in every map.  colors are written only with a colour image, confidences only when conf_iterations > 0.
+ *   - Counting: a map whose outputs are all NULL is only counted: n_vertices and n_faces are written and its capacities
+ *     are not checked, so that two calls give exactly sized buffers.  Otherwise a map whose counts exceed cap_vertices or
+ *     cap_faces fails the call with B200MVS_ERR_OVERFLOW and a message naming the first such map; every map's counts are
+ *     still written and no output buffer of any map is.
+ *   - Checks, all before anything is launched or written; a failure is B200MVS_ERR_INVALID_ARG with a message naming the
+ *     function, the map index and the field: n_maps < 0; maps NULL when n_maps > 0; conf_iterations < 0 (the reference's
+ *     "Invalid amount of iterations"); a NULL depth_dev; a width or height < 2 or more than 2^31 - 2 pixels (a map's
+ *     scan holds up to two faces per pixel in 32 bits); color_channels outside 1..4 with a colour image; an output
+ *     whose byte range (capacity x element size, vertex_ids width x height x 4) wraps the address space; a buffer that is host memory, memory of another device, or an output
+ *     or depth_dev not 4-byte aligned; a written range that overlaps any other written or read range of the call
+ *     (depth_dev and color_dev are read).  n_maps == 0 returns 0 and touches nothing.
+ *   - Streams: the work runs on cuda_stream (a cudaStream_t; NULL = the legacy default stream) after what is already
+ *     there, and the call returns when every output is written.  The counts are read back once, with one synchronisation;
+ *     with confidences, one more every 16 rings of a chunk whose border rings have not yet stopped.
+ *   - Memory: the maps go in order in chunks, each the longest run of consecutive maps of at most 2^28 pixels in all (a
+ *     larger map is a chunk of its own).  The workspace is allocated once per call and sized to the largest chunk: 17 B
+ *     per pixel, plus 4 B when a map with outputs has no vertex_ids, 12 B when one has no vertices (the vertices are
+ *     computed for every map with outputs) and 8 B when confidences are computed, plus the scan's temporary storage;
+ *     and a table of 224 B per map and 4 B per 256 pixels of a map.  Everything is freed before the call returns. */
+typedef struct b200mvs_dm_mesh {
+    /* input, read in place */
+    const float* depth_dev;           /* width x height floats on `device` */
+    int32_t width, height;            /* >= 2 each, width * height <= 2^31 - 2 */
+    float invproj[9];                 /* as b200mvs_depthmap_pointset */
+    const float* cam_to_world;        /* HOST, 16 floats row-major, or NULL */
+    const uint8_t* color_dev;         /* packed height x width x color_channels bytes on `device`, any alignment, or NULL */
+    int32_t color_channels;           /* 1..4 when color_dev != NULL */
+    /* outputs on `device`, NULL = not wanted */
+    uint32_t* vertex_ids;             /* width * height */
+    float* vertices;                  /* 3 floats per vertex */
+    float* colors;                    /* 4 floats per vertex */
+    uint32_t* faces;                  /* 3 per face */
+    float* normals;                   /* 3 floats per vertex */
+    float* confidences;               /* 1 float per vertex */
+    float* scales;                    /* 1 float per vertex */
+    uint64_t cap_vertices, cap_faces;
+    /* results */
+    uint64_t n_vertices, n_faces;
+} b200mvs_dm_mesh;
+int b200mvs_depthmap_pointset_device(int device, int n_maps, b200mvs_dm_mesh* maps, float dd_factor, int conf_iterations,
+                                     float scale_factor, void* cuda_stream);
+
 /* ---- the whole-scene point set of apps/scene2pset (scene2pset.cc:247-464) on the device ---- */
 /*
 

@@ -29,6 +29,7 @@ def _lib():
         L.b200mvs_depthmap_pointset.argtypes = [C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_int,
                                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                                 C.c_float, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.b200mvs_depthmap_pointset_device.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_float, C.c_int, C.c_float, C.c_void_p]
         L._dm_ready = True
     return L
 
@@ -137,10 +138,93 @@ def depthmap_cleanup_maps(dms, thres, out=None):
     return outs
 
 
+class DmMesh(C.Structure):
+    """b200mvs_dm_mesh (include/b200mvs.h): one map of b200mvs_depthmap_pointset_device."""
+    _fields_ = [("depth_dev", C.c_void_p), ("width", C.c_int32), ("height", C.c_int32), ("invproj", C.c_float * 9),
+                ("cam_to_world", C.c_void_p), ("color_dev", C.c_void_p), ("color_channels", C.c_int32),
+                ("vertex_ids", C.c_void_p), ("vertices", C.c_void_p), ("colors", C.c_void_p), ("faces", C.c_void_p),
+                ("normals", C.c_void_p), ("confidences", C.c_void_p), ("scales", C.c_void_p),
+                ("cap_vertices", C.c_uint64), ("cap_faces", C.c_uint64), ("n_vertices", C.c_uint64), ("n_faces", C.c_uint64)]
+
+
+def _per_map(what, v, n):
+    v = [None] * n if v is None else list(v)
+    if len(v) != n:
+        raise ValueError("%d %s for %d maps" % (len(v), what, n))
+    return v
+
+
+def depthmap_pointset_maps(dms, invprojs, colors=None, cam_to_world=None, dd_factor: float = DD_FACTOR_DEFAULT,
+                           with_normals: bool = False, conf_iterations: int = 0, scale_factor: Optional[float] = None):
+    """depthmap_pointset on each map of a batch of torch CUDA tensors, e.g. the depth maps of
+    Scene.reconstruct(on_device=True): float32, contiguous, H x W, all on one device.  invprojs: one 3x3 (or 9) inverse
+    projection per map.  colors: None, or one uint8 H x W or H x W x C CUDA tensor (or None) per map, e.g.
+    Scene.level(v, s, on_device=True).  cam_to_world: None, or one 4x4 host matrix (or None) per map.
+    Two library calls (b200mvs_depthmap_pointset_device) on the device's current stream: one counts, one fills new,
+    exactly sized tensors.  Returns one dict per map with the keys of depthmap_pointset but device_ms, each value a CUDA
+    tensor or None when skipped; vertex_ids and faces are torch.uint32 (torch.int32 with the same bits on a torch
+    without uint32)."""
+    import torch
+    dms = list(dms)
+    dev = _device_maps("dms", dms)
+    n = len(dms)
+    ips = np.ascontiguousarray(invprojs, np.float32)
+    if ips.size != 9 * n:
+        raise ValueError("invprojs must hold one 3x3 matrix per map (%d maps)" % n)
+    ips = ips.reshape(n, 9)
+    cols = _per_map("colour images", colors, n)
+    ctws = [None if c is None else np.ascontiguousarray(c, np.float32).reshape(16) for c in _per_map("cam_to_world", cam_to_world, n)]
+    meshes = (DmMesh * max(n, 1))()
+    for j, (d, c) in enumerate(zip(dms, cols)):
+        m = meshes[j]
+        m.depth_dev, m.height, m.width = d.data_ptr(), d.shape[0], d.shape[1]
+        m.invproj[:] = [float(x) for x in ips[j]]
+        m.cam_to_world = None if ctws[j] is None else ctws[j].ctypes.data
+        if c is not None:
+            if not _is_cuda(c) or c.device != dev or c.dtype != torch.uint8 or c.dim() not in (2, 3) or not c.is_contiguous():
+                raise ValueError("colors[%d] must be a contiguous uint8 CUDA tensor on %s" % (j, dev))
+            if tuple(c.shape[:2]) != tuple(d.shape):
+                raise ValueError("Color image dimension mismatch (map %d)" % j)
+            m.color_dev, m.color_channels = c.data_ptr(), 1 if c.dim() == 2 else c.shape[2]
+    index, _, _, _, stream = _batch(dms, dev)
+    L = _lib()
+
+    def call():
+        _check(L.b200mvs_depthmap_pointset_device(index, n, meshes, float(dd_factor), int(conf_iterations),
+                                                  float(scale_factor if scale_factor is not None else 0.0), stream))
+    call()
+    u32 = getattr(torch, "uint32", torch.int32)
+    out = []
+    for j, (d, c) in enumerate(zip(dms, cols)):
+        m = meshes[j]
+        nv, nf = int(m.n_vertices), int(m.n_faces)
+        f32 = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)      # noqa: E731
+        r = dict(vertex_ids=torch.empty(tuple(d.shape), dtype=u32, device=dev), vertices=f32(nv, 3),
+                 colors=None if c is None else f32(nv, 4), faces=torch.empty((nf, 3), dtype=u32, device=dev),
+                 normals=f32(nv, 3) if with_normals else None, confidences=f32(nv) if conf_iterations > 0 else None,
+                 scales=f32(nv) if scale_factor is not None else None)
+        for k, t in r.items():
+            setattr(m, k, None if t is None else t.data_ptr())
+        m.cap_vertices, m.cap_faces = nv, nf
+        out.append(r)
+    call()
+    return out
+
+
+def depthmap_triangulate_maps(dms, invprojs, colors=None, cam_to_world=None, dd_factor: float = DD_FACTOR_DEFAULT):
+    """depthmap_triangulate on each map of a batch of torch CUDA tensors: depthmap_pointset_maps without the per-vertex
+    attributes.  Returns one dict per map with vertex_ids, vertices, colors (or None) and faces."""
+    keys = ("vertex_ids", "vertices", "colors", "faces")
+    return [{k: r[k] for k in keys} for r in depthmap_pointset_maps(dms, invprojs, colors, cam_to_world, dd_factor)]
+
+
 def depthmap_triangulate(dm: np.ndarray, invproj: np.ndarray, dd_factor: float = DD_FACTOR_DEFAULT,
                          cam_to_world: Optional[np.ndarray] = None, color: Optional[np.ndarray] = None, device: int = 0):
     """mve::geom::depthmap_triangulate (depthmap.cc:196-375). Returns dict(vertex_ids [H,W] uint32, vertices [V,3], colors [V,4]
-    or None, faces [F,3] uint32, device_ms)."""
+    or None, faces [F,3] uint32, device_ms).  dm (and color) may be torch CUDA tensors (`device` is then theirs): the
+    result is the dict of depthmap_triangulate_maps, CUDA tensors without device_ms."""
+    if _is_cuda(dm):
+        return depthmap_triangulate_maps([dm], [invproj], [color], [cam_to_world], dd_factor)[0]
     dm = np.ascontiguousarray(dm, np.float32)
     h, w = dm.shape
     ip = np.ascontiguousarray(invproj, np.float32).reshape(9)
@@ -167,7 +251,11 @@ def depthmap_pointset(dm: np.ndarray, invproj: np.ndarray, dd_factor: float = DD
                       cam_to_world: Optional[np.ndarray] = None, color: Optional[np.ndarray] = None,
                       with_normals: bool = True, conf_iterations: int = 4, scale_factor: Optional[float] = 2.5, device: int = 0):
     """The per-view work of apps/scene2pset (scene2pset.cc:264-358): triangulation + vertex normals + boundary confidences +
-    scale values. Returns the dict of depthmap_triangulate plus normals [V,3], confidences [V], scales [V] (None when skipped)."""
+    scale values. Returns the dict of depthmap_triangulate plus normals [V,3], confidences [V], scales [V] (None when skipped).
+    dm (and color) may be torch CUDA tensors (`device` is then theirs): the result is the dict of depthmap_pointset_maps."""
+    if _is_cuda(dm):
+        return depthmap_pointset_maps([dm], [invproj], [color], [cam_to_world], dd_factor, with_normals, conf_iterations,
+                                      scale_factor)[0]
     dm = np.ascontiguousarray(dm, np.float32)
     h, w = dm.shape
     ip = np.ascontiguousarray(invproj, np.float32).reshape(9)

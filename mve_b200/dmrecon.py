@@ -86,7 +86,7 @@ EXPORTS = ["b200mvs_default_settings", "b200mvs_create", "b200mvs_destroy", "b20
            "b200mvs_get_level", "b200mvs_global_view_selection", "b200mvs_optimize_patches", "b200mvs_reconstruct",
            "b200mvs_plan_views", "b200mvs_set_patch_mode", "b200mvs_depthmap_last_error", "b200mvs_depthmap_confidence_clean",
            "b200mvs_depthmap_cleanup", "b200mvs_depthmap_triangulate", "b200mvs_depthmap_pointset",
-           "b200mvs_depthmap_confidence_clean_device", "b200mvs_depthmap_cleanup_device",
+           "b200mvs_depthmap_confidence_clean_device", "b200mvs_depthmap_cleanup_device", "b200mvs_depthmap_pointset_device",
            "b200mvs_set_image_source", "b200mvs_memory_stats", "b200mvs_working_set", "b200mvs_plan_batches",
            "b200mvs_set_frontier_capacity", "b200mvs_frontier_info", "b200mvs_plan_stats", "b200mvs_pset_create", "b200mvs_pset_destroy",
            "b200mvs_pset_add_view", "b200mvs_pset_clip_masks", "b200mvs_pset_get_info", "b200mvs_pset_read",
