@@ -188,9 +188,24 @@ int b200mvs_set_view_distortion(b200mvs_ctx* ctx, int view_id, float k2, float k
  * apply it, with or without a budget.  Masks leave view selection, plans, b200mvs_working_set, b200mvs_plan_batches,
  * b200mvs_optimize_patches and the sampling of neighbour views as they are, and add no device bytes (the mask travels
  * in the batch's own map arrays).  It is not the clip of b200mvs_pset_clip_masks, which deletes points afterwards.
- * The mask is copied; NULL clears it (w and h are then ignored).  Plans and pyramids are kept, and it works in a
+ * The mask is copied to the host; NULL clears it (w and h are then ignored).  A view has one mask: this call replaces a
+ * mask of b200mvs_set_view_mask_device and frees its device block.  Plans and pyramids are kept, and it works in a
  * planning context, where it only stores the mask.  A bad view id, or w or h < 1 with a mask: B200MVS_ERR_INVALID_ARG. */
 int b200mvs_set_view_mask(b200mvs_ctx* ctx, int view_id, const uint8_t* mask_or_null, int w, int h);
+/* The same mask read from DEVICE memory on the context's device: row y of the w x h bytes starts at
+ * mask_dev + y * row_pitch (row_pitch >= w).  Every reconstruction gives exactly what b200mvs_set_view_mask gives for the
+ * same bytes: the same maps, seeds, counters and points on every route, with or without a budget.
+ *   - The bytes are copied into a packed w x h block of the view in device memory, after an event recorded on cuda_stream
+ *     (NULL = the legacy default stream); the call returns when the copy is done, so the source may then be reused.
+ *   - The block is taken from the context's budget and counted in b200mvs_memory.fixed (and resident) until the mask is
+ *     cleared or replaced, or the context is destroyed.  A mask that does not fit gives B200MVS_ERR_NO_MEMORY and leaves
+ *     the view's previous mask in place.
+ *   - A launch resamples the mask into the batch's map arrays on the device: no host loop and no upload.
+ *   - It replaces a host mask of b200mvs_set_view_mask; NULL clears either kind (w, h and row_pitch are then ignored).
+ *   - B200MVS_ERR_INVALID_ARG, naming the function and the field, before anything is copied: a bad view id, w or h < 1,
+ *     row_pitch < w, a planning context, and a mask_dev in host memory (pinned or pageable) or on another device. */
+int b200mvs_set_view_mask_device(b200mvs_ctx* ctx, int view_id, const uint8_t* mask_dev_or_null, int w, int h,
+                                 int64_t row_pitch, void* cuda_stream);
 /* mve::Bundle::Features (bundle.h:51-60) as position + CSR list of referencing view ids. */
 int b200mvs_set_features(b200mvs_ctx* ctx, int n_features, const float* pos,
                          const int32_t* ref_offsets, const int32_t* ref_view_ids);
@@ -585,6 +600,16 @@ int b200mvs_pset_add_view_device(b200mvs_pset* ps, int view_id, const float* dep
  * Callable once per handle; no view can be added afterwards. */
 int b200mvs_pset_clip_masks(b200mvs_pset* ps, int n_masks, const uint8_t* const* masks, const int32_t* widths,
                             const int32_t* heights, const b200mvs_pset_camera* cams, uint64_t* num_filtered);
+/* The same with the masks in DEVICE memory on the handle's device, read in place: row y of mask m starts at
+ * masks_dev[m] + y * row_pitches[m] (row_pitches[m] >= widths[m]).  The point set, num_filtered and the per-list rule are
+ * b200mvs_pset_clip_masks' for the same mask bytes, on either kind of handle.  Its checks, plus row_pitches and the
+ * device-buffer check of b200mvs_reconstruct_device at any alignment, all run before anything is launched, and a rejected
+ * call changes nothing.  The work waits for an event recorded on cuda_stream (NULL = the legacy default stream) at entry,
+ * and the call returns when the set is clipped; ms_mask adds the device time of the clip and the compaction.  No device
+ * memory beyond the set remains after the call. */
+int b200mvs_pset_clip_masks_device(b200mvs_pset* ps, int n_masks, const uint8_t* const* masks_dev, const int32_t* widths,
+                                   const int32_t* heights, const int64_t* row_pitches, const b200mvs_pset_camera* cams,
+                                   void* cuda_stream, uint64_t* num_filtered);
 int b200mvs_pset_get_info(b200mvs_pset* ps, b200mvs_pset_info* out);
 /* Copies the point set out; NULL skips an array.  vertices / normals 3 floats, colours 4 floats (n_colors of them),
  * values and confidences 1 float per point.  Normals, values and confidences exist when the options asked for them. */

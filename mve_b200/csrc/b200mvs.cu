@@ -98,13 +98,15 @@ struct HostView {
     float flen = 0, paspect = 1, pp[2] = {0.5f, 0.5f}, rot[9], trans[3];
     float k2 = 0, k4 = 0;          // radial distortion of the images it is given (b200mvs_set_view_distortion)
     std::vector<uint8_t> mask;     // reconstruction mask, mask_w x mask_h, 0 = background (b200mvs_set_view_mask); empty: none
+    DevBuf<uint8_t> mask_dev;      // ... or the same in device memory (b200mvs_set_view_mask_device); at most one of the two
     int mask_w = 0, mask_h = 0;
     float campos[3];
     float w2c[12];
     std::vector<HostLevel> lv;
     DevBuf<uchar4> pyr;            // one allocation for every level: the RGBX8 images, then their quad images
     uint64_t last_use = 0;         // eviction order: least recently used first
-    explicit HostView(b200mvs_ctx* ctx) : pyr(ctx) {}
+    explicit HostView(b200mvs_ctx* ctx) : mask_dev(ctx), pyr(ctx) {}
+    bool masked() const { return !mask.empty() || mask_dev.p; }
 };
 
 // Device bytes of a view's pyramid: every level of buildPyramid, RGBX8 + quad image (16 B) per texel at a pitch of 4 texels
@@ -117,14 +119,14 @@ size_t pyramid_bytes(const HostView& v)
 
 // b200mvs_set_view_mask: the mask column (row) under the centre of column (row) x of a map n pixels wide (high), for a
 // mask m pixels wide (high): floor((2x+1) m / 2n)
-int mask_coord(int x, int n, int m) { return (int)((2ll * x + 1) * m / (2ll * n)); }
-// whether pixel (x, y) of view v's W x H map is background; a pixel outside the map is not
+__host__ __device__ inline int mask_coord(int x, int n, int m) { return (int)((2ll * x + 1) * m / (2ll * n)); }
+// whether pixel (x, y) of view v's W x H map is background under its host mask; a pixel outside the map is not
 bool background(const HostView& v, int W, int H, int x, int y)
 {
     if (v.mask.empty() || x < 0 || y < 0 || x >= W || y >= H) return false;
     return v.mask[(size_t)mask_coord(y, H, v.mask_h) * v.mask_w + mask_coord(x, W, v.mask_w)] == 0;
 }
-// bg[y * W + x] = 1 where pixel (x, y) of view v's W x H map is background, else 0 (v has a mask)
+// bg[y * W + x] = 1 where pixel (x, y) of view v's W x H map is background, else 0 (v has a host mask)
 void mark_background(const HostView& v, int W, int H, unsigned char* bg)
 {
     std::vector<int> col(W);
@@ -365,12 +367,15 @@ void release_workspace(b200mvs_ctx* ctx)
 }
 
 // Allocations that do not depend on the batch: view table, sRGB table, settings, frontier control block and the two
-// upload staging buffers, bounded by the largest registered image at 4 channels.
+// upload staging buffers, bounded by the largest registered image at 4 channels, and the device reconstruction masks.
 uint64_t fixed_bytes(const b200mvs_ctx* ctx)
 {
-    size_t stage = 0;
-    for (const HostView& v : ctx->views) if (v.valid) stage = std::max(stage, (size_t)v.w * v.h * 4);
-    return sizeof(ViewParams) * ctx->views.size() + 256 * sizeof(float) + sizeof(DevSettings) + sizeof(FrontierCtl) + 2 * stage;
+    size_t stage = 0, masks = 0;
+    for (const HostView& v : ctx->views) {
+        if (v.valid) stage = std::max(stage, (size_t)v.w * v.h * 4);
+        masks += v.mask_dev.bytes();
+    }
+    return sizeof(ViewParams) * ctx->views.size() + 256 * sizeof(float) + sizeof(DevSettings) + sizeof(FrontierCtl) + 2 * stage + masks;
 }
 
 bool has_source(const b200mvs_ctx* ctx) { return ctx->fetch || ctx->fetch_device; }
@@ -833,6 +838,28 @@ __global__ void k_mask_background(float* __restrict__ conf, unsigned char* __res
     if (p >= n || !bg[p]) return;
     bg[p] = 0;
     conf[p] = INFINITY;
+}
+// The bytes of `bg` for one view's W x H map from its device mask (b200mvs_set_view_mask_device), as mark_background
+// makes them from a host mask
+__global__ void k_mark_background(const uint8_t* __restrict__ mask, int mw, int mh, int W, int H, unsigned char* __restrict__ bg)
+{
+    const int x = blockIdx.x * blockDim.x + threadIdx.x;
+    const int y = blockIdx.y * blockDim.y + threadIdx.y;
+    if (x >= W || y >= H) return;
+    bg[(size_t)y * W + x] = mask[(size_t)mask_coord(y, H, mh) * mw + mask_coord(x, W, mw)] == 0;
+}
+// The device mask of one view for k_seed_background, with the size of the view's map
+struct SeedMask { const uint8_t* mask; int mw, mh, W, H; };
+// bg[i] = whether seed i, pixel (x, y) of view `view` of seeds[i] = (x, y, view, -), lies on a background pixel; a seed
+// outside the map does not (background())
+__global__ void k_seed_background(const SeedMask* __restrict__ views, const int4* __restrict__ seeds, size_t n, unsigned char* __restrict__ bg)
+{
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int4 q = seeds[i];
+    const SeedMask V = views[q.z];
+    bg[i] = q.x >= 0 && q.y >= 0 && q.x < V.W && q.y < V.H &&
+            V.mask[(size_t)mask_coord(q.y, V.H, V.mh) * V.mw + mask_coord(q.x, V.W, V.mw)] == 0;
 }
 // after the launch: background pixels leave the device as unfilled ones, conf = 0
 __global__ void k_unmask_background(float* __restrict__ conf, size_t n)
@@ -1930,8 +1957,50 @@ int b200mvs_set_view_mask(b200mvs_ctx* ctx, int id, const uint8_t* mask, int w, 
     if (id < 0 || id >= (int)ctx->views.size() || (mask && (w < 1 || h < 1)))
         return fail(B200MVS_ERR_INVALID_ARG, "b200mvs_set_view_mask: bad arguments");
     HostView& v = ctx->views[id];
+    if (v.mask_dev.p) {
+        CK(cudaSetDevice(ctx->device));
+        v.mask_dev.release();
+    }
     if (!mask) { v.mask.clear(); v.mask.shrink_to_fit(); v.mask_w = v.mask_h = 0; return 0; }
     v.mask.assign(mask, mask + (size_t)w * h);
+    v.mask_w = w; v.mask_h = h;
+    return 0;
+}
+
+int b200mvs_set_view_mask_device(b200mvs_ctx* ctx, int id, const uint8_t* mask_dev, int w, int h, int64_t row_pitch, void* cuda_stream)
+{
+    static const char* fn = "b200mvs_set_view_mask_device";
+    if (!ctx) return fail(B200MVS_ERR_INVALID_ARG, "%s: null context", fn);
+    std::lock_guard<std::mutex> lk(ctx->mtx);
+    const int nv = (int)ctx->views.size();
+    if (id < 0 || id >= nv) return fail(B200MVS_ERR_INVALID_ARG, "%s: view_id is %d, not in 0..%d", fn, id, nv - 1);
+    HostView& v = ctx->views[id];
+    if (!mask_dev) {
+        if (v.mask_dev.p) { CK(cudaSetDevice(ctx->device)); v.mask_dev.release(); }
+        v.mask.clear(); v.mask.shrink_to_fit(); v.mask_w = v.mask_h = 0;
+        return 0;
+    }
+    if (w < 1) return fail(B200MVS_ERR_INVALID_ARG, "%s: w is %d, must be at least 1", fn, w);
+    if (h < 1) return fail(B200MVS_ERR_INVALID_ARG, "%s: h is %d, must be at least 1", fn, h);
+    if (row_pitch < w) return fail(B200MVS_ERR_INVALID_ARG, "%s: row_pitch is %lld, less than w (%d)", fn, (long long)row_pitch, w);
+    if (ctx->device == B200MVS_DEVICE_NONE)
+        return fail(B200MVS_ERR_INVALID_ARG, "%s: mask_dev cannot be read by a planning context (B200MVS_DEVICE_NONE), which has no device", fn);
+    CK(cudaSetDevice(ctx->device));
+    int rc = check_device_buffer(fn, "mask_dev", mask_dev, ctx->device, 1);
+    if (rc) return rc;
+    // the new block is filled before the old one goes, so a mask that does not fit leaves the previous one in place
+    DevBuf<uint8_t> block(ctx);
+    if (block.reserve((size_t)w * h) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(B200MVS_ERR_NO_MEMORY, "%s: a %d x %d mask does not fit the device budget", fn, w, h);
+    }
+    cudaStream_t st = ctx->stream.get();
+    if ((rc = wait_for_stream(ctx->ev_caller.get(), cuda_stream, st))) return rc;
+    CK(cudaMemcpy2DAsync(block.p, (size_t)w, mask_dev, (size_t)row_pitch, (size_t)w, (size_t)h, cudaMemcpyDeviceToDevice, st));
+    CK(cudaStreamSynchronize(st));
+    std::swap(v.mask_dev.p, block.p);
+    std::swap(v.mask_dev.cap, block.cap);
+    v.mask.clear(); v.mask.shrink_to_fit();
     v.mask_w = w; v.mask_h = h;
     return 0;
 }
@@ -2522,6 +2591,53 @@ int grow_frontier(b200mvs_ctx* ctx, const FrontierCtl& c, FrontierParams& P, siz
     return 0;
 }
 
+// Whether each seed of each reference view lies on a background pixel of the view's reconstruction mask at level s.scale:
+// bg[j][i] for seed i of refs[j], empty for a view without a mask.  Host masks are read on the host; the seeds of every
+// view with a device mask are looked up by one k_seed_background launch.
+int seed_background(b200mvs_ctx* ctx, const b200mvs_settings& s, int n_refs, const int32_t* refs, const std::vector<HostPlan>& plans,
+                    std::vector<std::vector<char>>& bg)
+{
+    bg.assign(n_refs, {});
+    std::vector<SeedMask> views;
+    std::vector<int4> seeds;
+    for (int j = 0; j < n_refs; ++j) {
+        const HostView& v = ctx->views[refs[j]];
+        const HostLevel& L = v.lv[s.scale];
+        const std::vector<PL::SeedOut>& q = plans[j].seeds;
+        if (!v.mask.empty()) {
+            bg[j].resize(q.size());
+            for (size_t i = 0; i < q.size(); ++i) bg[j][i] = background(v, L.w, L.h, q[i].x, q[i].y);
+        } else if (v.mask_dev.p && !q.empty()) {
+            for (const PL::SeedOut& p : q) seeds.push_back(make_int4(p.x, p.y, (int)views.size(), 0));
+            views.push_back(SeedMask{v.mask_dev.p, v.mask_w, v.mask_h, L.w, L.h});
+        }
+    }
+    if (seeds.empty()) return 0;
+    DevBuf<SeedMask> d_views(ctx);
+    DevBuf<int4> d_seeds(ctx);
+    DevBuf<unsigned char> d_bg(ctx);
+    CK(d_views.reserve(views.size()));
+    CK(d_seeds.reserve(seeds.size()));
+    CK(d_bg.reserve(seeds.size()));
+    cudaStream_t st = ctx->stream.get();
+    CK(cudaMemcpyAsync(d_views.p, views.data(), sizeof(SeedMask) * views.size(), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_seeds.p, seeds.data(), sizeof(int4) * seeds.size(), cudaMemcpyHostToDevice, st));
+    k_seed_background<<<(unsigned)((seeds.size() + 255) / 256), 256, 0, st>>>(d_views.p, d_seeds.p, seeds.size(), d_bg.p);
+    CK(cudaGetLastError());
+    std::vector<unsigned char> flags(seeds.size());
+    CK(cudaMemcpyAsync(flags.data(), d_bg.p, flags.size(), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    size_t at = 0;
+    for (int j = 0; j < n_refs; ++j) {
+        const HostView& v = ctx->views[refs[j]];
+        if (!v.mask.empty() || !v.mask_dev.p) continue;
+        const size_t n = plans[j].seeds.size();
+        bg[j].assign(flags.begin() + at, flags.begin() + at + n);
+        at += n;
+    }
+    return 0;
+}
+
 // Where a reconstruction's maps go: the caller's buffers (buffer_sink) or a point set.  Right after a group's launch,
 // unless the whole group was cancelled, each view j gets its width and height in sizes[j] (when set) and, unless it was
 // cancelled, take(j, job) runs while the group's maps and pyramids are resident.  take may allocate up to bytes(w, h)
@@ -2535,9 +2651,9 @@ struct MapSink {
 
 // One frontier launch over the reference views refs[j], j in js (at most MAX_GROUP_VIEWS): makes room for the pyramids
 // they need within the budget (`reserve` bytes kept free for the sink), loads the missing ones, runs, hands the maps to
-// `sink`.  Accumulates `stats`; marks the views that ended cancelled in `view_cancelled`.
+// `sink`.  Accumulates `stats`; marks the views that ended cancelled in `view_cancelled`.  seed_bg: seed_background's flags.
 int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int>& js, const int32_t* refs,
-              const std::vector<HostPlan>& plans, const MapSink* sink, uint64_t reserve,
+              const std::vector<HostPlan>& plans, const std::vector<std::vector<char>>& seed_bg, const MapSink* sink, uint64_t reserve,
               b200mvs_progress* progress, b200mvs_stats* stats, int32_t* failed_view, std::vector<char>& view_cancelled)
 {
     // `if (progress.cancelled) return` at the head of every stage (dmrecon.cc:100-104,336): a group whose views were all
@@ -2588,10 +2704,11 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
         jobs[k].tiles_x = (jobs[k].W + 15) / 16;
         jobs[k].tile_base = (long long)n_tiles;
         n_tiles += (size_t)jobs[k].tiles_x * ((jobs[k].H + 15) / 16);
-        const HostView& rv = ctx->views[refs[j]];
-        masked = masked || !rv.mask.empty();
-        for (const PL::SeedOut& q : plans[j].seeds) {
-            if (background(rv, jobs[k].W, jobs[k].H, q.x, q.y)) continue;
+        masked = masked || ctx->views[refs[j]].masked();
+        const std::vector<char>& bg = seed_bg[j];
+        for (size_t i = 0; i < plans[j].seeds.size(); ++i) {
+            if (!bg.empty() && bg[i]) continue;
+            const PL::SeedOut& q = plans[j].seeds[i];
             // a seed outside the image fails in the PatchSampler ctor (patch_sampler.cc:47-50); keep it so that the
             // processed count matches, the kernel rejects it by the same bounds test
             const int x = std::min(std::max(q.x, -1), 0xFFFE), y = std::min(std::max(q.y, -1), 0xFFFE);
@@ -2629,11 +2746,18 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
         CK(cudaMemsetAsync(slots, 0xFF, total_px * 4, st));
         if (masked) {
             // the background bytes of the masked views travel in the zeroed normal maps (12 bytes per pixel, one used),
-            // so a mask adds no device memory; k_mask_background zeroes them again
+            // so a mask adds no memory to the batch; k_mask_background zeroes them again.  A host mask is resampled on the
+            // host and uploaded, a device mask is resampled in place by k_mark_background.
             unsigned char* bg_dev = reinterpret_cast<unsigned char*>(normal);
             std::vector<unsigned char> bg;
             for (int k = 0; k < n_refs; ++k) {
                 const HostView& rv = ctx->views[refs[js[k]]];
+                if (rv.mask_dev.p) {
+                    const dim3 blk(32, 8), grd((jobs[k].W + 31) / 32, (jobs[k].H + 7) / 8);
+                    k_mark_background<<<grd, blk, 0, st>>>(rv.mask_dev.p, rv.mask_w, rv.mask_h, jobs[k].W, jobs[k].H, bg_dev + px_off[k]);
+                    CK(cudaGetLastError());
+                    continue;
+                }
                 if (rv.mask.empty()) continue;
                 bg.resize((size_t)jobs[k].W * jobs[k].H);
                 mark_background(rv, jobs[k].W, jobs[k].H, bg.data());
@@ -2812,13 +2936,12 @@ int reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const i
             for (int g : plans[j].gsel)
                 if (!ctx->views[g].has_image) { if (failed_view) *failed_view = refs[j]; return fail(B200MVS_ERR_INVALID_ARG, "color image of view %d (selected neighbour of view %d) is not loaded", g, refs[j]); }
         }
-    if (stats)
-        for (int j = 0; j < n_refs; ++j) {
-            const HostView& rv = ctx->views[refs[j]];
-            const HostLevel& L = rv.lv[s->scale];
-            for (const PL::SeedOut& q : plans[j].seeds) stats->n_seeds_processed += !background(rv, L.w, L.h, q.x, q.y);
-        }
     CK(cudaSetDevice(ctx->device));
+    std::vector<std::vector<char>> seed_bg;
+    if ((rc = seed_background(ctx, *s, n_refs, refs, plans, seed_bg))) return rc;
+    if (stats)
+        for (int j = 0; j < n_refs; ++j)
+            stats->n_seeds_processed += plans[j].seeds.size() - std::count(seed_bg[j].begin(), seed_bg[j].end(), 1);
 
     // ---- groups that fit the budget, one frontier launch each ----
     uint64_t reserve = 0;
@@ -2838,7 +2961,7 @@ int reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const i
     for (int g = 0; g < n_groups; ++g) {
         std::vector<int> js;
         for (int j = 0; j < n_refs; ++j) if (group_of[j] == g) js.push_back(j);
-        if ((rc = run_group(ctx, s, js, refs, plans, sink, reserve, progress, stats, failed_view, view_cancelled))) return rc;
+        if ((rc = run_group(ctx, s, js, refs, plans, seed_bg, sink, reserve, progress, stats, failed_view, view_cancelled))) return rc;
     }
     if (std::all_of(view_cancelled.begin(), view_cancelled.end(), [](char c) { return c != 0; }))
         return fail(B200MVS_ERR_CANCELLED, "reconstruction cancelled");

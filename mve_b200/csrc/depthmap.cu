@@ -937,9 +937,10 @@ __global__ void k_vertex_pixels(const unsigned* __restrict__ vids, int w, size_t
 //   c_r = fma(z, W[r][2], fma(x, W[r][0], y * W[r][1])) + W[r][3]          (Matrix4f::mult(v, 1), contracted)
 //   p0 = fma(c2, K2, fma(K0, c0, c1 * K1)), p1 = fma(c2, K5, fma(K3, c0, c1 * K4)), p2 = fma(c2, K8, fma(c0, K6, c1 * K7))
 //   x = p0 / p2, y = p1 / p2 (true divisions); outside when x < 0 || y < 0 || x >= w || y >= h.
-struct MaskCam { float W[12]; float K[9]; int w, h; unsigned long long offset; };
+// Row y of a mask starts at mask + y * pitch, in the block the host masks are uploaded to or in the caller's device memory.
+struct MaskCam { float W[12]; float K[9]; int w, h; const unsigned char* mask; long long pitch; };
 __global__ void k_mask_clip(const float* __restrict__ verts, size_t n, const MaskCam* __restrict__ cams, int n_masks,
-                            const unsigned char* __restrict__ masks, unsigned char* __restrict__ del)
+                            unsigned char* __restrict__ del)
 {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -956,7 +957,7 @@ __global__ void k_mask_clip(const float* __restrict__ verts, size_t n, const Mas
         const float px = __fdiv_rn(p0, p2), py = __fdiv_rn(p1, p2);
         if (px < 0.0f || py < 0.0f || px >= (float)C.w || py >= (float)C.h) continue;
         if (isnan(px) || isnan(py)) continue;       // the reference would index its mask at INT_MIN
-        if (masks[C.offset + (size_t)(int)py * C.w + (int)px] == 0) d = 1;
+        if (C.mask[(int)py * C.pitch + (int)px] == 0) d = 1;
     }
     del[i] = d;
 }
@@ -1699,24 +1700,42 @@ int b200mvs_pset_add_view_device(b200mvs_pset* ps, int view_id, const float* dep
     return add_view(ps, view_id, depth_dev, w, h, Color{color_dev, color_channels, color_channels, w}, *cam, out);
 }
 
-int b200mvs_pset_clip_masks(b200mvs_pset* ps, int n_masks, const uint8_t* const* masks, const int32_t* widths, const int32_t* heights,
-                            const b200mvs_pset_camera* cams, uint64_t* num_filtered)
+} // extern "C"
+
+namespace {
+
+// b200mvs_pset_clip_masks (`fn`: host masks, uploaded into one block) and b200mvs_pset_clip_masks_device (in_place: device
+// masks with row pitches, read where they are after the work of cuda_stream)
+int clip_masks(const char* fn, bool in_place, b200mvs_pset* ps, int n_masks, const uint8_t* const* masks, const int32_t* widths,
+               const int32_t* heights, const int64_t* pitches, const b200mvs_pset_camera* cams, void* cuda_stream, uint64_t* num_filtered)
 {
-    if (!ps || n_masks < 0 || (n_masks && (!masks || !widths || !heights || !cams)))
-        return fail(B200MVS_ERR_INVALID_ARG, "b200mvs_pset_clip_masks: null argument");
+    if (!ps || n_masks < 0 || (n_masks && (!masks || !widths || !heights || !cams || (in_place && !pitches))))
+        return fail(B200MVS_ERR_INVALID_ARG, "%s: null argument", fn);
     if (ps->opt.correspondence)
-        return fail(B200MVS_ERR_INVALID_ARG, "b200mvs_pset_clip_masks: correspondence needs every vertex (no mask clipping)");
-    for (int m = 0; m < n_masks; ++m)
+        return fail(B200MVS_ERR_INVALID_ARG, "%s: correspondence needs every vertex (no mask clipping)", fn);
+    for (int m = 0; m < n_masks; ++m) {
         if (!masks[m] || widths[m] < 1 || heights[m] < 1 || cams[m].flen == 0.0f)
-            return fail(B200MVS_ERR_INVALID_ARG, "b200mvs_pset_clip_masks: bad mask, size or camera");
-    if (ps->clipped) return fail(B200MVS_ERR_INVALID_ARG, "b200mvs_pset_clip_masks: the masks have been applied already");
+            return fail(B200MVS_ERR_INVALID_ARG, "%s: bad mask, size or camera", fn);
+        if (in_place && pitches[m] < widths[m])
+            return fail(B200MVS_ERR_INVALID_ARG, "%s: row_pitches[%d] is %lld, less than widths[%d] (%d)", fn, m, (long long)pitches[m], m,
+                        widths[m]);
+    }
+    if (ps->clipped) return fail(B200MVS_ERR_INVALID_ARG, "%s: the masks have been applied already", fn);
     Work& W = ps->W;
     Lists& S = ps->set;
     TempBuf d_masks(W), d_cams(W), d_verts(W), d_del(W), before(W), scan_tmp(W), out(W);
     CK(cudaSetDevice(ps->device));
+    if (in_place) {
+        for (int m = 0; m < n_masks; ++m)
+            if (const int rc = check_device_buffer(fn, "masks_dev[" + std::to_string(m) + "]", masks[m], ps->device, 1)) return rc;
+        // the handle's work runs on the legacy default stream, after what the caller enqueued on its stream
+        CK(W.events());
+        if (const int rc = wait_for_stream(W.ev[4], cuda_stream, cudaStreamLegacy)) return rc;
+    }
     ps->clipped = true;
     const uint64_t np = S.n[Lists::VERTS];
     std::vector<MaskCam> mc((size_t)n_masks);
+    std::vector<size_t> offset((size_t)n_masks);
     size_t bytes = 0;
     for (int m = 0; m < n_masks; ++m) {
         MaskCam& C = mc[m];
@@ -1726,8 +1745,11 @@ int b200mvs_pset_clip_masks(b200mvs_pset* ps, int n_masks, const uint8_t* const*
                               c.rot[6], c.rot[7], c.rot[8], c.trans[2]};
         std::memcpy(C.W, Wm, sizeof(Wm));
         fill_calibration(c.flen, c.paspect, c.ppoint[0], c.ppoint[1], (float)widths[m], (float)heights[m], C.K, nullptr);
-        C.w = widths[m]; C.h = heights[m]; C.offset = bytes;
-        bytes += (size_t)widths[m] * heights[m];
+        C.w = widths[m]; C.h = heights[m];
+        C.mask = in_place ? masks[m] : nullptr;           // a host mask's place in d_masks is known once it is allocated
+        C.pitch = in_place ? pitches[m] : widths[m];
+        offset[m] = bytes;
+        if (!in_place) bytes += (size_t)widths[m] * heights[m];
     }
     uint64_t filtered = 0;
     if (n_masks && np) {
@@ -1760,8 +1782,10 @@ int b200mvs_pset_clip_masks(b200mvs_pset* ps, int n_masks, const uint8_t* const*
         // ms_mask (b200mvs_pset_info): a host set's time includes every transfer, a device set's only the work in place
         CK(W.events());
         if (!dev) CK(cudaEventRecord(W.ev[2]));
-        for (int m = 0; m < n_masks; ++m)
-            CK(cudaMemcpy(P<unsigned char>(d_masks) + mc[m].offset, masks[m], (size_t)widths[m] * heights[m], cudaMemcpyHostToDevice));
+        for (int m = 0; m < n_masks && !in_place; ++m) {
+            mc[m].mask = P<unsigned char>(d_masks) + offset[m];
+            CK(cudaMemcpy(P<unsigned char>(d_masks) + offset[m], masks[m], (size_t)widths[m] * heights[m], cudaMemcpyHostToDevice));
+        }
         CK(cudaMemcpy(d_cams.p, mc.data(), mc.size() * sizeof(MaskCam), cudaMemcpyHostToDevice));
         if (dev) CK(cudaEventRecord(W.ev[2]));
         for (uint64_t at = 0; at < np; at += CHUNK) {
@@ -1769,7 +1793,7 @@ int b200mvs_pset_clip_masks(b200mvs_pset* ps, int n_masks, const uint8_t* const*
             const float* v = static_cast<const float*>(S.p[Lists::VERTS]) + 3 * at;
             unsigned char* d = P<unsigned char>(d_del) + (dev ? at : 0);
             if (!dev) { CK(cudaMemcpy(d_verts.p, v, k * 12, cudaMemcpyHostToDevice)); v = P<float>(d_verts); }
-            k_mask_clip<<<(unsigned)((k + 255) / 256), 256>>>(v, k, P<MaskCam>(d_cams), n_masks, P<unsigned char>(d_masks), d);
+            k_mask_clip<<<(unsigned)((k + 255) / 256), 256>>>(v, k, P<MaskCam>(d_cams), n_masks, d);
             CK(cudaGetLastError());
             if (!dev) CK(cudaMemcpy(del.data() + at, d, k, cudaMemcpyDeviceToHost));
         }
@@ -1819,6 +1843,24 @@ int b200mvs_pset_clip_masks(b200mvs_pset* ps, int n_masks, const uint8_t* const*
     }
     if (num_filtered) *num_filtered = filtered;
     return 0;
+}
+
+} // namespace
+
+extern "C" {
+
+int b200mvs_pset_clip_masks(b200mvs_pset* ps, int n_masks, const uint8_t* const* masks, const int32_t* widths, const int32_t* heights,
+                            const b200mvs_pset_camera* cams, uint64_t* num_filtered)
+{
+    return clip_masks("b200mvs_pset_clip_masks", false, ps, n_masks, masks, widths, heights, nullptr, cams, nullptr, num_filtered);
+}
+
+int b200mvs_pset_clip_masks_device(b200mvs_pset* ps, int n_masks, const uint8_t* const* masks_dev, const int32_t* widths,
+                                   const int32_t* heights, const int64_t* row_pitches, const b200mvs_pset_camera* cams,
+                                   void* cuda_stream, uint64_t* num_filtered)
+{
+    return clip_masks("b200mvs_pset_clip_masks_device", true, ps, n_masks, masks_dev, widths, heights, row_pitches, cams, cuda_stream,
+                      num_filtered);
 }
 
 int b200mvs_pset_get_info(b200mvs_pset* ps, b200mvs_pset_info* out)

@@ -319,6 +319,8 @@ def _pset_lib():
         L.b200mvs_pset_add_view_device.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                                    C.POINTER(_PsetCamera), C.c_void_p, C.POINTER(_PsetView)]
         L.b200mvs_pset_clip_masks.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
+        L.b200mvs_pset_clip_masks_device.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                     C.c_void_p, C.POINTER(C.c_uint64)]
         L.b200mvs_pset_get_info.argtypes = [C.c_void_p, C.POINTER(_PsetInfo)]
         L.b200mvs_pset_read.argtypes = [C.c_void_p] + [C.c_void_p] * 5
         L.b200mvs_pset_read_correspondence.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
@@ -358,11 +360,54 @@ def _view_record(view_id, r):
                 first_index=int(r.first_index))
 
 
-def _finish(L, h, o, masks, per_view, device=None):
+def _cuda_masks(masks, device):
+    """Whether the masks of scene_pointset are CUDA tensors (on the handle's `device`, else ValueError) or all host
+    arrays; a mix raises ValueError.  Checked before any library call."""
+    if not masks:
+        return False
+    cuda = [_is_cuda(m["mask"]) for m in masks]
+    if any(cuda) and not all(cuda):
+        raise ValueError("masks must be all CUDA tensors or all host arrays, not a mix")
+    if cuda[0]:
+        import torch
+        dev = torch.device("cuda", device) if device >= 0 else None
+        for m in masks:
+            if m["mask"].device != dev:
+                raise ValueError("a CUDA mask must be on the point set's device %s, not %s" % (dev, m["mask"].device))
+    return cuda[0]
+
+
+def _clip_device_masks(L, h, masks, device):
+    """b200mvs_pset_clip_masks_device with CUDA tensor masks, read in place after the work of the current stream."""
+    import torch
+    ts = []
+    for m in masks:
+        t = m["mask"]
+        if t.dim() != 2:
+            raise ValueError("masks must have one channel")
+        t = t.to(torch.uint8)
+        if (t.shape[1] > 1 and t.stride(1) != 1) or (t.shape[0] > 1 and t.stride(0) < t.shape[1]):
+            t = t.contiguous()
+        ts.append(t)
+    ptrs = (C.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
+    ws = np.array([t.shape[1] for t in ts], np.int32)
+    hs = np.array([t.shape[0] for t in ts], np.int32)
+    pitches = np.array([t.stride(0) if t.shape[0] > 1 else t.shape[1] for t in ts], np.int64)
+    cams = (_PsetCamera * len(ts))(*[_camera(m["camera"]) for m in masks])
+    stream = torch.cuda.current_stream(torch.device("cuda", device)).cuda_stream
+    nf = C.c_uint64(0)
+    _check(L.b200mvs_pset_clip_masks_device(h, len(ts), ptrs, _p(ws), _p(hs), _p(pitches), cams, C.c_void_p(stream), C.byref(nf)))
+    return int(nf.value)
+
+
+def _finish(L, h, o, masks, per_view, device=None, mask_device=None):
     """Clips the handle's points with `masks` and reads the point set out (the result of scene_pointset): numpy arrays, or
-    with `device` (a handle's device index) torch CUDA tensors on that device, read on its current stream."""
+    with `device` (a handle's device index) torch CUDA tensors on that device, read on its current stream.  mask_device:
+    the handle's device when the masks are CUDA tensors (_cuda_masks)."""
     num_filtered = 0
-    if masks:
+    if masks and mask_device is not None:
+        num_filtered = _clip_device_masks(L, h, masks, mask_device)
+    elif masks:
         ms = [np.ascontiguousarray(m["mask"], np.uint8) for m in masks]
         if any(m.ndim != 2 for m in ms):
             raise ValueError("masks must have one channel")
@@ -423,7 +468,9 @@ def scene_pointset(views, options=None, masks=None, device: int = 0, on_device: 
     (b200mvs_pset_add_view_device, after the work of the current stream) and gives the same points as its host copy.
     options: with_normals, with_conf, with_scale, poisson_normals, correspondence, aabb ((min xyz), (max xyz)) or None,
     min_valid_fraction (0), scale_factor (2.5), dd_factor (5), conf_iterations (4).
-    masks: dicts with mask [H, W] uint8 (one channel) and camera; the points any of them marks 0 are deleted.
+    masks: dicts with mask [H, W] uint8 (one channel) and camera; the points any of them marks 0 are deleted.  The masks
+    may be torch CUDA tensors on `device`, all of them or none: they are read in place after the work of the current
+    stream (b200mvs_pset_clip_masks_device), with either value of on_device and the same results.
 
     Returns dict(vertices [N, 3], normals [N, 3] or None, colors [M, 4] (M < N when a view had no colour image),
     values [N] or None, confidences [N] or None, views (per input view: id, added, fraction, n_points, first_index),
@@ -435,6 +482,7 @@ def scene_pointset(views, options=None, masks=None, device: int = 0, on_device: 
     (b200mvs_pset_read_device), with the shapes and dtypes above; the pixels are torch.uint32 (torch.int32 with the same
     bits on a torch without uint32).  views, correspondence views, num_filtered and info stay host values."""
     o, opt = _options(options)
+    cuda_masks = _cuda_masks(masks, device)
     L = _pset_lib()
     h = _create(L, device, opt, on_device)
     try:
@@ -455,7 +503,7 @@ def scene_pointset(views, options=None, masks=None, device: int = 0, on_device: 
             cam = _camera(v["camera"])
             _check(L.b200mvs_pset_add_view(h, int(v["id"]), _p(dm), dm.shape[1], dm.shape[0], _p(col), cch, C.byref(cam), C.byref(r)))
             per_view.append(_view_record(v["id"], r))
-        return _finish(L, h, o, masks, per_view, device if on_device else None)
+        return _finish(L, h, o, masks, per_view, device if on_device else None, device if cuda_masks else None)
     finally:
         L.b200mvs_pset_destroy(h)
 
@@ -496,6 +544,7 @@ def reconstruct_pointset(scene, settings, ref_views, options=None, masks=None, p
     scene_pointset (on_device: the set never leaves the scene's device); progress as for Scene.reconstruct.  Returns
     (the dict of scene_pointset, dmrecon.Stats)."""
     o, opt = _options(options)
+    cuda_masks = _cuda_masks(masks, scene.device)
     L = _pset_lib()
     refs = np.asarray(ref_views, np.int32)
     h = C.c_void_p()
@@ -514,7 +563,8 @@ def reconstruct_pointset(scene, settings, ref_views, options=None, masks=None, p
                 msg += " (view %d)" % failed.value
             raise dmrecon.B200MVSError(rc, msg, failed.value)
         per_view = [_view_record(v, recs[j]) for j, v in enumerate(refs.tolist())]
-        return _finish(L, h, o, masks, per_view, scene.device if on_device else None), stats
+        return _finish(L, h, o, masks, per_view, scene.device if on_device else None,
+                       scene.device if cuda_masks else None), stats
     finally:
         if h.value:
             L.b200mvs_pset_destroy(h)

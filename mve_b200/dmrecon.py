@@ -92,7 +92,8 @@ EXPORTS = ["b200mvs_default_settings", "b200mvs_create", "b200mvs_destroy", "b20
            "b200mvs_pset_add_view", "b200mvs_pset_clip_masks", "b200mvs_pset_get_info", "b200mvs_pset_read",
            "b200mvs_pset_read_correspondence", "b200mvs_pset_add_reconstruction", "b200mvs_reconstruct_device",
            "b200mvs_get_level_device", "b200mvs_pset_add_view_device", "b200mvs_pset_create_on_device", "b200mvs_pset_read_device",
-           "b200mvs_set_view_distortion", "b200mvs_set_image_source_device", "b200mvs_set_view_mask"]
+           "b200mvs_set_view_distortion", "b200mvs_set_image_source_device", "b200mvs_set_view_mask",
+           "b200mvs_set_view_mask_device", "b200mvs_pset_clip_masks_device"]
 
 ERR_INVALID_ARG = -1
 ERR_CUDA = -2
@@ -206,6 +207,7 @@ def lib():
     L.b200mvs_set_features.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     L.b200mvs_set_view_distortion.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_float]
     L.b200mvs_set_view_mask.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int]
+    L.b200mvs_set_view_mask_device.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_void_p]
     L.b200mvs_set_view_camera.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
     L.b200mvs_num_levels.argtypes = [C.c_void_p, C.c_int]
     L.b200mvs_get_level.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -424,16 +426,23 @@ class Scene:
         imports images unchanged.  A changed value drops the view's resident pyramid; cameras are unchanged."""
         self._check(self._lib.b200mvs_set_view_distortion(self._h, view_id, float(k2), float(k4)))
 
-    def set_view_mask(self, view_id: int, mask):
+    def set_view_mask(self, view_id: int, mask, on_device: bool = False):
         """Reconstruction mask of a reference view (b200mvs_set_view_mask): an H x W uint8 array, 0 = background, the
         convention of scene2pset -m; a numpy array or a torch tensor (a CUDA tensor is copied to the host).  None clears it.
         reconstruct(), reconstruct(on_device=True) and reconstruct_pointset() then never seed, queue or optimise a
         background pixel: it ends unfilled (depth, conf, dz, normal 0, view ids -1) and yields no point.  Pixel (x, y) of a
         W x H map is background when mask pixel ((2x+1) * mask_w // 2W, (2y+1) * mask_h // 2H) is 0, so the mask may have
         the photo's size or any level's.  This differs from the `masks=` of reconstruct_pointset(), which deletes points of
-        the finished point set (scene2pset -m) after every pixel has been reconstructed."""
+        the finished point set (scene2pset -m) after every pixel has been reconstructed.
+        on_device: the mask is an H x W torch.uint8 CUDA tensor on the scene's device, copied on the device after the
+        work of its current stream (b200mvs_set_view_mask_device), with the same results.  Its rows may be pitched (a
+        tensor whose rows are not dense is made contiguous first); the copy is kept in device memory, counted in
+        memory_stats().fixed, until the mask is cleared or replaced.  Anything else raises ValueError."""
         if mask is None:
             self._check(self._lib.b200mvs_set_view_mask(self._h, view_id, None, 0, 0))
+            return
+        if on_device:
+            self._set_view_mask_device(view_id, mask)
             return
         if hasattr(mask, "detach"):                  # a torch tensor, on the host or a device
             mask = mask.detach().cpu().numpy()
@@ -442,6 +451,24 @@ class Scene:
             raise ValueError("a view mask is an H x W uint8 array, not %s %s" % (m.dtype, m.shape))
         m = np.ascontiguousarray(m)
         self._check(self._lib.b200mvs_set_view_mask(self._h, view_id, _p(m), m.shape[1], m.shape[0]))
+
+    def _set_view_mask_device(self, view_id: int, mask):
+        torch = _torch()
+        if (not isinstance(mask, torch.Tensor) or mask.dtype != torch.uint8 or mask.dim() != 2 or not mask.is_cuda
+                or (self.device != DEVICE_NONE and mask.device != torch.device(self._torch_device()))):
+            where = "the scene's device" if self.device == DEVICE_NONE else self._torch_device()
+            raise ValueError("an on-device view mask is an H x W torch.uint8 tensor on %s, not %s" % (
+                where, "%s %s on %s" % (mask.dtype, tuple(mask.shape), mask.device) if isinstance(mask, torch.Tensor)
+                else type(mask).__name__))
+        h, w = mask.shape
+        if h < 1 or w < 1:
+            raise ValueError("an on-device view mask must not be empty, not %d x %d" % (h, w))
+        if (w > 1 and mask.stride(1) != 1) or (h > 1 and mask.stride(0) < w):
+            mask = mask.contiguous()
+        pitch = mask.stride(0) if h > 1 else w
+        stream = torch.cuda.current_stream(mask.device).cuda_stream
+        self._check(self._lib.b200mvs_set_view_mask_device(self._h, view_id, C.c_void_p(mask.data_ptr()), w, h, pitch,
+                                                           C.c_void_p(stream)))
 
     def set_features(self, pos: np.ndarray, refs: Sequence[np.ndarray]):
         """mve::Bundle::Features (bundle.h:51-60)."""
