@@ -325,6 +325,36 @@ int b200mvs_reconstruct_device(b200mvs_ctx* ctx, const b200mvs_settings* s, int 
                                b200mvs_maps* maps_dev, void* cuda_stream, b200mvs_progress* progress, b200mvs_stats* stats,
                                int32_t* failed_view_or_null);
 
+/* ---- per-entry pyramid levels: views of different sizes (apps/dmrecon --max-pixels, dmrecon.cc:89-111,299-302) or one
+ *      view at several levels (scene2pset -F2, -F3) in one call ----
+ * The *_levels forms of b200mvs_reconstruct, b200mvs_reconstruct_device, b200mvs_pset_add_reconstruction,
+ * b200mvs_working_set and b200mvs_plan_batches take levels[j] (n_refs entries) next to ref_views[j]:
+ *   - Levels.  Entry j reconstructs ref_views[j] at pyramid level levels[j]; s->scale is not read.  Every other rule is
+ *     that of the call without levels: settings checks, codes and messages, progress and cancellation per entry, stats
+ *     summed over entries, groups, the budget, the image source, the sink and the stream rule.  A call with every
+ *     levels[j] == s->scale is the call without levels.
+ *   - Maps.  An entry's maps (depth, conf, dz, normal, view_ids) are bit for bit those of a single-level call of that view
+ *     at that level, whatever the other entries and levels of the call; b200mvs_maps.width/height are those of the
+ *     entry's level.  Masks are per view and resampled to each entry's map size by the rule of b200mvs_set_view_mask.
+ *   - Checks.  levels == NULL, a level < 0 or past the view's pyramid ("Invalid scale factor", failed_view_or_null
+ *     receives the view) give B200MVS_ERR_INVALID_ARG; the 65535-pixels-per-side limit applies to each entry's level.
+ *   - Repeated views.  A view may appear at several levels, but a (view, level) pair only once: a repeat gives
+ *     B200MVS_ERR_INVALID_ARG with a message naming the view and the level before anything runs.  All entries of a view
+ *     share its one pyramid: it is counted once in the working set, pinned once per group and fetched once when its
+ *     group needs it.
+ *   - Plans.  Prepared plans (b200mvs_plan_views) stay stored one per view with their settings; an entry uses one when
+ *     the plan's settings equal s with scale = levels[j], and the other entries are planned in the call, once per
+ *     distinct level with that level's calibration, so selections and seeds are those of a single-level call.
+ *     b200mvs_plan_info counts entries.
+ *   - Groups.  Working set and groups work per entry, at the entry's pixel and seed counts; the 4000-views-per-group
+ *     limit counts entries. */
+int b200mvs_reconstruct_levels(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* ref_views,
+                               const int32_t* levels, b200mvs_maps* maps, b200mvs_progress* progress, b200mvs_stats* stats,
+                               int32_t* failed_view_or_null);
+int b200mvs_reconstruct_levels_device(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* ref_views,
+                                      const int32_t* levels, b200mvs_maps* maps_dev, void* cuda_stream,
+                                      b200mvs_progress* progress, b200mvs_stats* stats, int32_t* failed_view_or_null);
+
 /* ---- device memory budget: images loaded on demand (ImagePyramidCache::cleanup, image_pyramid.cc:134-155) ----
  * Without a source (the default) the context has no budget: no pyramid is evicted, so every one stays resident until the
  * context is destroyed, and b200mvs_reconstruct runs a batch of up to 4000 views in one launch. */
@@ -411,6 +441,13 @@ int b200mvs_working_set(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs,
  * (failed_view_or_null receives its id). */
 int b200mvs_plan_batches(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* ref_views,
                          uint64_t available, int32_t* group_of_ref, int32_t* failed_view_or_null);
+/* The two above with one pyramid level per entry (see b200mvs_reconstruct_levels): the maps, tiles and seeds of entry j
+ * are those of ref_views[j] at levels[j], and each view's pyramid is counted once however many entries it has.  With every
+ * levels[j] == s->scale they return what b200mvs_working_set and b200mvs_plan_batches return. */
+int b200mvs_working_set_levels(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* ref_views,
+                               const int32_t* levels, uint64_t* bytes);
+int b200mvs_plan_batches_levels(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* ref_views,
+                                const int32_t* levels, uint64_t available, int32_t* group_of_ref, int32_t* failed_view_or_null);
 
 /* ---- consumers of the depth maps, on the device (SURVEY.md 8f rank 2 and 3).  Stateless: host buffers in, host buffers
  *      out (the *_device forms: device buffers in and out), `device` = CUDA device ordinal.  Errors: negative code, message
@@ -654,6 +691,13 @@ int b200mvs_pset_add_reconstruction(b200mvs_pset* ps, b200mvs_ctx* ctx, const b2
                                     int n_refs, const int32_t* ref_views,
                                     b200mvs_progress* progress, b200mvs_stats* stats,
                                     int32_t* failed_view_or_null, b200mvs_pset_view* views_out_or_null);
+/* The same with one pyramid level per entry (see b200mvs_reconstruct_levels): entry j appends what b200mvs_pset_add_view
+ * appends for the depth map of ref_views[j] at levels[j], the view's level image levels[j] (b200mvs_get_level) and its
+ * camera, in entry order; views_out_or_null has one record per entry. */
+int b200mvs_pset_add_reconstruction_levels(b200mvs_pset* ps, b200mvs_ctx* ctx, const b200mvs_settings* s,
+                                           int n_refs, const int32_t* ref_views, const int32_t* levels,
+                                           b200mvs_progress* progress, b200mvs_stats* stats,
+                                           int32_t* failed_view_or_null, b200mvs_pset_view* views_out_or_null);
 
 #ifdef __cplusplus
 }

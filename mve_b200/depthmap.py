@@ -326,6 +326,8 @@ def _pset_lib():
         L.b200mvs_pset_read_correspondence.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         L.b200mvs_pset_add_reconstruction.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                                                       C.c_void_p, C.c_void_p, C.c_void_p]
+        L.b200mvs_pset_add_reconstruction_levels.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L._pset_ready = True
     return L
 
@@ -536,17 +538,21 @@ def _add_device_view(L, h, v):
     return _view_record(v["id"], r)
 
 
-def reconstruct_pointset(scene, settings, ref_views, options=None, masks=None, progress=None, on_device: bool = False):
+def reconstruct_pointset(scene, settings, ref_views, options=None, masks=None, progress=None, on_device: bool = False,
+                         scales=None):
     """dmrecon and scene2pset in one call (b200mvs_pset_add_reconstruction): reconstructs the reference views of
     `scene` (a dmrecon.Scene) and builds their point set on the device, each view's depth map and colours (its pyramid
     level settings.scale) staying on the device.  Equal to scene.reconstruct(...) followed by scene_pointset of the maps
     with the level images and the registered cameras, in ref_views order.  options, masks and on_device as for
-    scene_pointset (on_device: the set never leaves the scene's device); progress as for Scene.reconstruct.  Returns
+    scene_pointset (on_device: the set never leaves the scene's device); progress as for Scene.reconstruct.
+    scales: one pyramid level per reference view instead of settings.scale (b200mvs_pset_add_reconstruction_levels);
+    a view may appear at several levels, and each entry adds the points of its map and its level image.  Returns
     (the dict of scene_pointset, dmrecon.Stats)."""
     o, opt = _options(options)
     cuda_masks = _cuda_masks(masks, scene.device)
     L = _pset_lib()
     refs = np.asarray(ref_views, np.int32)
+    levels = dmrecon.levels_array(scales, len(refs))
     h = C.c_void_p()
     # a planning context has no device to make a handle on: the call itself rejects the context
     if scene.device != dmrecon.DEVICE_NONE:
@@ -555,8 +561,12 @@ def reconstruct_pointset(scene, settings, ref_views, options=None, masks=None, p
         recs = (_PsetView * max(1, len(refs)))()
         stats = dmrecon.Stats()
         failed = C.c_int32(-1)
-        rc = L.b200mvs_pset_add_reconstruction(h, scene._h, C.byref(settings), len(refs), _p(refs), progress, C.byref(stats),
-                                               C.byref(failed), recs)
+        if levels is None:
+            rc = L.b200mvs_pset_add_reconstruction(h, scene._h, C.byref(settings), len(refs), _p(refs), progress,
+                                                   C.byref(stats), C.byref(failed), recs)
+        else:
+            rc = L.b200mvs_pset_add_reconstruction_levels(h, scene._h, C.byref(settings), len(refs), _p(refs), _p(levels),
+                                                          progress, C.byref(stats), C.byref(failed), recs)
         if rc != 0:
             msg = L.b200mvs_last_error(None).decode()
             if failed.value >= 0:

@@ -13,6 +13,7 @@
 //                              under the reference's embedding names (depth-L<s>, dz-L<s>, conf-L<s>, undist-L<s>),
 //                              writePlyFile / plyPath through the reference's own save_ply_view, same log lines, Progress
 //                              updated live while the kernel runs, cancellation of a running view -> RECON_CANCELLED
+#include <algorithm>
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -122,7 +123,13 @@ void throw_for(int rc, const std::string& msg)
     throw std::runtime_error(msg);     // B200MVS_ERR_GLOBAL_VS ("Global View Selection failed"), CUDA errors, overflow
 }
 
-bool same_settings(const b200mvs_settings& a, const b200mvs_settings& b) { return std::memcmp(&a, &b, sizeof(a)) == 0; }
+// Requests whose settings differ at most in the scale run in one b200mvs_reconstruct_levels call, each at its own scale
+// (--max-pixels gives views of different sizes different scales, apps/dmrecon/dmrecon.cc:89-111,299-302)
+bool same_settings_but_scale(b200mvs_settings a, b200mvs_settings b)
+{
+    a.scale = b.scale = 0;
+    return std::memcmp(&a, &b, sizeof(a)) == 0;
+}
 
 // Image source of a device context: the library loads the colour images a batch needs (loadColorImage, dmrecon.cc:78,
 // 238-240) and evicts pyramids to stay within the device budget (ImagePyramidCache::cleanup, image_pyramid.cc:134-155).
@@ -234,11 +241,14 @@ void run_batch(DeviceCtx& D, std::vector<Request*> batch)
     }
     while (!live.empty()) {
         const size_t n = live.size();
-        std::vector<int32_t> refs(n);
+        std::vector<int32_t> refs(n), levels(n);
         std::vector<b200mvs_maps> maps(n);
         std::vector<b200mvs_progress> prog(n);
         std::memset(prog.data(), 0, sizeof(b200mvs_progress) * n);
-        for (size_t i = 0; i < n; ++i) { refs[i] = live[i]->ref; maps[i] = live[i]->maps; live[i]->progress->status = mvs::RECON_QUEUE; }
+        for (size_t i = 0; i < n; ++i) {
+            refs[i] = live[i]->ref; levels[i] = live[i]->settings.scale; maps[i] = live[i]->maps;
+            live[i]->progress->status = mvs::RECON_QUEUE;
+        }
         // relay: live progress out, cancel requests in (Progress is read/written without locks in the reference too,
         // fancy_progress_printer.cc:84-91, apps/umve/viewinspect/imageoperations.cc:177-184)
         std::atomic<bool> stop(false);
@@ -254,7 +264,8 @@ void run_batch(DeviceCtx& D, std::vector<Request*> batch)
         });
         b200mvs_stats stats;
         int32_t failed = -1;
-        const int rc = b200mvs_reconstruct(D.ctx, &live[0]->settings, (int)n, refs.data(), maps.data(), prog.data(), &stats, &failed);
+        const int rc = b200mvs_reconstruct_levels(D.ctx, &live[0]->settings, (int)n, refs.data(), levels.data(), maps.data(),
+                                                  prog.data(), &stats, &failed);
         stop = true;
         relay.join();
         if (rc == 0 || rc == B200MVS_ERR_CANCELLED) {
@@ -456,10 +467,16 @@ DMRecon::start()
                 seen = D.arrivals;
                 if (std::chrono::steady_clock::now() - t_open > std::chrono::milliseconds(D.planners > 0 ? 250 : 30)) break;
             }
+            // one batch: the requests that share the first one's settings up to the scale and its embedding, each
+            // (view, scale) once
             std::vector<Request*> batch;
             std::vector<Request*> rest;
-            for (Request* r : D.pending)
-                (batch.empty() || (same_settings(r->settings, batch[0]->settings) && r->embedding == batch[0]->embedding) ? batch : rest).push_back(r);
+            for (Request* r : D.pending) {
+                const bool joins = batch.empty() ||
+                    (same_settings_but_scale(r->settings, batch[0]->settings) && r->embedding == batch[0]->embedding &&
+                     std::none_of(batch.begin(), batch.end(), [&](const Request* q) { return q->ref == r->ref && q->settings.scale == r->settings.scale; }));
+                (joins ? batch : rest).push_back(r);
+            }
             D.pending.swap(rest);
             D.last_batch = batch.size();
             lock.unlock();
