@@ -206,6 +206,38 @@ int b200mvs_set_view_mask(b200mvs_ctx* ctx, int view_id, const uint8_t* mask_or_
  *     row_pitch < w, a planning context, and a mask_dev in host memory (pinned or pageable) or on another device. */
 int b200mvs_set_view_mask_device(b200mvs_ctx* ctx, int view_id, const uint8_t* mask_dev_or_null, int w, int h,
                                  int64_t row_pitch, void* cuda_stream);
+/* Prior depth map of a reference view: region growing starts from it as well as from the SfM features.  depth is w x h
+ * floats, row-major, in MVE's convention: the distance from the camera centre along the pixel's unit ray, as in a
+ * depth-L<s> embedding.  That value does not depend on the level, so it is never rescaled.
+ *   - Which pixels seed: an entry that reconstructs the view at level `scale` with a W x H map has the candidate pixels
+ *     x = 2 + stride i <= W - 3 and y = 2 + stride k <= H - 3 (a pixel nearer the edge always fails in the PatchSampler
+ *     ctor): nx = W >= 5 ? (W - 5) / stride + 1 : 0 columns and, by the same rule, ny rows.  Candidate (x, y) reads prior
+ *     pixel (floor((2x+1) w / 2W), floor((2y+1) h / 2H)), the pixel rule of b200mvs_set_view_mask, and is a seed when
+ *     that value is finite and > 0 and the pixel is not background under the view's mask.
+ *   - A prior seed is what a feature seed is: no local views, conf 0, the prior depth and dz 0, so the seed round runs
+ *     the full local view selection for it.  Prior seeds come after every feature seed of the launch; per pixel the
+ *     most confident seed wins and the earlier one wins a tie, so a feature seed beats a prior seed of equal confidence.
+ *     n_seeds_processed and n_seeds_success count the prior seeds that were made.
+ *   - Every reconstruction entry point applies it: b200mvs_reconstruct[_levels][_device] and
+ *     b200mvs_pset_add_reconstruction[_levels].  b200mvs_optimize_patches does not.
+ *   - b200mvs_working_set[_levels] and b200mvs_plan_batches[_levels] count an entry's candidate bound nx x ny as seeds,
+ *     as they count feature seeds; a view without a prior gives what it gives without this call.  A launch group whose
+ *     feature seeds and candidate bounds exceed 2^31 - 1 fails with B200MVS_ERR_INVALID_ARG before anything runs
+ *     (failed_view receives one of its views).
+ *   - The prior is copied into a packed w x h float block of the view in device memory, taken from the context's budget
+ *     and counted in b200mvs_memory.fixed (and resident) until it is cleared or replaced, or the context is destroyed.
+ *     A prior that does not fit gives B200MVS_ERR_NO_MEMORY and leaves the previous one in place.  A new prior replaces
+ *     the old one and frees its block; NULL clears it (w, h and stride are then ignored).  Plans and pyramids are kept.
+ *   - B200MVS_ERR_INVALID_ARG, naming the function and the field, before anything is copied: a bad view id, w or h < 1,
+ *     stride outside 1..65535, and a planning context (the prior lives on the device). */
+int b200mvs_set_view_prior(b200mvs_ctx* ctx, int view_id, const float* depth_or_null, int w, int h, int stride);
+/* The same prior read from DEVICE memory on the context's device: row y of the w x h floats starts at
+ * depth_dev + y * row_pitch bytes.  Every reconstruction gives exactly what b200mvs_set_view_prior gives for the same
+ * values.  The copy runs after an event recorded on cuda_stream (NULL = the legacy default stream), and the call returns
+ * when it is done, so the source may then be reused.  Its checks, plus row_pitch < 4 w or not a multiple of 4, and a
+ * depth_dev in host memory (pinned or pageable), on another device or not 4-byte aligned. */
+int b200mvs_set_view_prior_device(b200mvs_ctx* ctx, int view_id, const float* depth_dev_or_null, int w, int h,
+                                  int64_t row_pitch, int stride, void* cuda_stream);
 /* mve::Bundle::Features (bundle.h:51-60) as position + CSR list of referencing view ids. */
 int b200mvs_set_features(b200mvs_ctx* ctx, int n_features, const float* pos,
                          const int32_t* ref_offsets, const int32_t* ref_view_ids);
@@ -416,7 +448,8 @@ int b200mvs_set_image_source_device(b200mvs_ctx* ctx, b200mvs_device_fetch_fn fe
 typedef struct b200mvs_memory {
     uint64_t budget;              /* 0 = no source installed (no limit)                                           */
     uint64_t fixed;               /* bytes that do not depend on the batch: view table, sRGB table, settings and frontier
-                                     control block, two upload staging buffers of the largest registered image (bound) */
+                                     control block, two upload staging buffers of the largest registered image (bound),
+                                     device masks and priors                                                          */
     uint64_t resident;            /* device bytes the context holds now                                          */
     uint64_t peak;                /* maximum of `resident` since creation or since the source was installed        */
     uint64_t n_loads;             /* images fetched through the source                                           */

@@ -10,6 +10,7 @@
 #include "undistort.cuh"
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdarg>
 #include <cstddef>
@@ -100,12 +101,14 @@ struct HostView {
     std::vector<uint8_t> mask;     // reconstruction mask, mask_w x mask_h, 0 = background (b200mvs_set_view_mask); empty: none
     DevBuf<uint8_t> mask_dev;      // ... or the same in device memory (b200mvs_set_view_mask_device); at most one of the two
     int mask_w = 0, mask_h = 0;
+    DevBuf<float> prior;           // prior depth map, prior_w x prior_h (b200mvs_set_view_prior[_device]); null: none
+    int prior_w = 0, prior_h = 0, prior_stride = 0;
     float campos[3];
     float w2c[12];
     std::vector<HostLevel> lv;
     DevBuf<uchar4> pyr;            // one allocation for every level: the RGBX8 images, then their quad images
     uint64_t last_use = 0;         // eviction order: least recently used first
-    explicit HostView(b200mvs_ctx* ctx) : mask_dev(ctx), pyr(ctx) {}
+    explicit HostView(b200mvs_ctx* ctx) : mask_dev(ctx), prior(ctx), pyr(ctx) {}
     bool masked() const { return !mask.empty() || mask_dev.p; }
 };
 
@@ -137,6 +140,17 @@ void mark_background(const HostView& v, int W, int H, unsigned char* bg)
         if (v.mask_w == W) for (int x = 0; x < W; ++x) out[x] = row[x] == 0;          // col[x] == x: no gather
         else for (int x = 0; x < W; ++x) out[x] = row[col[x]] == 0;
     }
+}
+
+// b200mvs_set_view_prior: the candidate columns (rows) of a map n pixels wide (high) at `stride`, x = 2 + stride i <= n - 3;
+// a pixel nearer the edge fails in the PatchSampler ctor (patch_sampler.cc:47-50)
+__host__ __device__ inline int prior_cells(int n, int stride) { return n >= 5 ? (n - 5) / stride + 1 : 0; }
+// the candidate bound nx x ny of view v's prior at level `scale`: the most seeds it can add to an entry; 0 without a prior
+uint64_t prior_bound(const HostView& v, int scale)
+{
+    if (!v.prior.p) return 0;
+    const HostLevel& L = v.lv[scale];
+    return (uint64_t)prior_cells(L.w, v.prior_stride) * (uint64_t)prior_cells(L.h, v.prior_stride);
 }
 
 struct HostPlan {                    // what DMRecon::start computes on the host before the queue runs (dmrecon.cc:179-292)
@@ -367,13 +381,14 @@ void release_workspace(b200mvs_ctx* ctx)
 }
 
 // Allocations that do not depend on the batch: view table, sRGB table, settings, frontier control block and the two
-// upload staging buffers, bounded by the largest registered image at 4 channels, and the device reconstruction masks.
+// upload staging buffers, bounded by the largest registered image at 4 channels, the device reconstruction masks and the
+// prior depth maps.
 uint64_t fixed_bytes(const b200mvs_ctx* ctx)
 {
     size_t stage = 0, masks = 0;
     for (const HostView& v : ctx->views) {
         if (v.valid) stage = std::max(stage, (size_t)v.w * v.h * 4);
-        masks += v.mask_dev.bytes();
+        masks += v.mask_dev.bytes() + v.prior.bytes();
     }
     return sizeof(ViewParams) * ctx->views.size() + 256 * sizeof(float) + sizeof(DevSettings) + sizeof(FrontierCtl) + 2 * stage + masks;
 }
@@ -860,6 +875,22 @@ __global__ void k_seed_background(const SeedMask* __restrict__ views, const int4
     const SeedMask V = views[q.z];
     bg[i] = q.x >= 0 && q.y >= 0 && q.x < V.W && q.y < V.H &&
             V.mask[(size_t)mask_coord(q.y, V.H, V.mh) * V.mw + mask_coord(q.x, V.W, V.mw)] == 0;
+}
+// The prior seeds of one entry (b200mvs_set_view_prior): candidate c = (i, k) of the nx x ny grid is pixel
+// (2 + stride i, 2 + stride k) of the entry's W x H map; it reads prior pixel (mask_coord(x, W, pw), mask_coord(y, H, ph))
+// and becomes a seed when that depth is finite and > 0 and the pixel is not background (conf = +inf after
+// k_mask_background).  Seeds are appended at out[*cursor] in whatever order the atomic gives.  That order cannot change a
+// map: every prior seed comes after the feature seeds of the launch, and the prior seeds of one entry lie on distinct
+// pixels, so the seed round's per-pixel rule (most confident first, then the earlier seed) resolves them alike in any order.
+__global__ void k_prior_seeds(const float* __restrict__ prior, int pw, int ph, int stride, int nx, size_t n, int W, int H,
+                              const float* __restrict__ conf, int job, Entry* __restrict__ out, unsigned long long* __restrict__ cursor)
+{
+    const size_t c = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= n) return;
+    const int x = 2 + stride * (int)(c % nx), y = 2 + stride * (int)(c / nx);
+    const float d = __ldg(prior + (size_t)mask_coord(y, H, ph) * pw + mask_coord(x, W, pw));
+    if (!(d > 0.f) || isinf(d) || isinf(conf[(size_t)y * W + x])) return;
+    out[atomicAdd(cursor, 1ull)] = make_entry(pack_xy(x, y), job, 4, 0.f, d, 0.f, 0.f, 0xFFFFFFFFu);
 }
 // after the launch: background pixels leave the device as unfilled ones, conf = 0
 __global__ void k_unmask_background(float* __restrict__ conf, size_t n)
@@ -2014,6 +2045,82 @@ int b200mvs_set_view_mask_device(b200mvs_ctx* ctx, int id, const uint8_t* mask_d
     return 0;
 }
 
+namespace {
+
+// The checks of both prior calls with a prior: 0 when it may be stored
+int check_prior(const char* fn, const b200mvs_ctx* ctx, int id, int w, int h, int stride)
+{
+    const int nv = (int)ctx->views.size();
+    if (id < 0 || id >= nv) return fail(B200MVS_ERR_INVALID_ARG, "%s: view_id is %d, not in 0..%d", fn, id, nv - 1);
+    if (w < 1) return fail(B200MVS_ERR_INVALID_ARG, "%s: w is %d, must be at least 1", fn, w);
+    if (h < 1) return fail(B200MVS_ERR_INVALID_ARG, "%s: h is %d, must be at least 1", fn, h);
+    if (stride < 1 || stride > 65535) return fail(B200MVS_ERR_INVALID_ARG, "%s: stride is %d, not in 1..65535", fn, stride);
+    if (ctx->device == B200MVS_DEVICE_NONE)
+        return fail(B200MVS_ERR_INVALID_ARG, "%s: depth cannot be stored by a planning context (B200MVS_DEVICE_NONE), which has no device", fn);
+    return 0;
+}
+
+// Copies a w x h prior (rows `pitch` bytes apart, `kind`) into a new block of view `id`, which then replaces the old one.
+// The new block is filled before the old one goes, so a prior that does not fit leaves the previous one in place.
+int store_prior(const char* fn, b200mvs_ctx* ctx, int id, const float* src, int w, int h, size_t pitch, int stride,
+                cudaMemcpyKind kind)
+{
+    HostView& v = ctx->views[id];
+    DevBuf<float> block(ctx);
+    if (block.reserve((size_t)w * h) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(B200MVS_ERR_NO_MEMORY, "%s: a %d x %d prior does not fit the device budget", fn, w, h);
+    }
+    cudaStream_t st = ctx->stream.get();
+    CK(cudaMemcpy2DAsync(block.p, (size_t)w * sizeof(float), src, pitch, (size_t)w * sizeof(float), (size_t)h, kind, st));
+    CK(cudaStreamSynchronize(st));
+    std::swap(v.prior.p, block.p);
+    std::swap(v.prior.cap, block.cap);
+    v.prior_w = w; v.prior_h = h; v.prior_stride = stride;
+    return 0;
+}
+
+// NULL prior: view `id` has none from now on
+int clear_prior(const char* fn, b200mvs_ctx* ctx, int id)
+{
+    const int nv = (int)ctx->views.size();
+    if (id < 0 || id >= nv) return fail(B200MVS_ERR_INVALID_ARG, "%s: view_id is %d, not in 0..%d", fn, id, nv - 1);
+    HostView& v = ctx->views[id];
+    if (v.prior.p) { CK(cudaSetDevice(ctx->device)); v.prior.release(); }
+    v.prior_w = v.prior_h = v.prior_stride = 0;
+    return 0;
+}
+
+} // namespace
+
+int b200mvs_set_view_prior(b200mvs_ctx* ctx, int id, const float* depth, int w, int h, int stride)
+{
+    static const char* fn = "b200mvs_set_view_prior";
+    if (!ctx) return fail(B200MVS_ERR_INVALID_ARG, "%s: null context", fn);
+    std::lock_guard<std::mutex> lk(ctx->mtx);
+    if (!depth) return clear_prior(fn, ctx, id);
+    if (int rc = check_prior(fn, ctx, id, w, h, stride)) return rc;
+    CK(cudaSetDevice(ctx->device));
+    return store_prior(fn, ctx, id, depth, w, h, (size_t)w * sizeof(float), stride, cudaMemcpyHostToDevice);
+}
+
+int b200mvs_set_view_prior_device(b200mvs_ctx* ctx, int id, const float* depth_dev, int w, int h, int64_t row_pitch, int stride,
+                                  void* cuda_stream)
+{
+    static const char* fn = "b200mvs_set_view_prior_device";
+    if (!ctx) return fail(B200MVS_ERR_INVALID_ARG, "%s: null context", fn);
+    std::lock_guard<std::mutex> lk(ctx->mtx);
+    if (!depth_dev) return clear_prior(fn, ctx, id);
+    if (int rc = check_prior(fn, ctx, id, w, h, stride)) return rc;
+    if (row_pitch < 4ll * w || row_pitch % 4)
+        return fail(B200MVS_ERR_INVALID_ARG, "%s: row_pitch is %lld, not a multiple of 4 of at least 4 w (%lld)", fn,
+                    (long long)row_pitch, 4ll * w);
+    CK(cudaSetDevice(ctx->device));
+    if (int rc = check_device_buffer(fn, "depth_dev", depth_dev, ctx->device, 4)) return rc;
+    if (int rc = wait_for_stream(ctx->ev_caller.get(), cuda_stream, ctx->stream.get())) return rc;
+    return store_prior(fn, ctx, id, depth_dev, w, h, (size_t)row_pitch, stride, cudaMemcpyDeviceToDevice);
+}
+
 int b200mvs_set_features(b200mvs_ctx* ctx, int n, const float* pos, const int32_t* off, const int32_t* ids)
 {
     if (!ctx) return B200MVS_ERR_INVALID_ARG;
@@ -2509,14 +2616,14 @@ int plan_batch(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const in
     return 0;
 }
 
-// the workspace of reference view `ref` at level `scale`
+// the workspace of reference view `ref` at level `scale` with n_seeds feature seeds and the candidate bound of its prior
 Workspace view_workspace(const b200mvs_ctx* ctx, const b200mvs_settings& s, int scale, int ref, size_t n_seeds)
 {
     const HostLevel& L = ctx->views[ref].lv[scale];
     Workspace w(s, ctx->frontier_cap);
     w.px = (size_t)L.w * L.h;
     w.tiles = (size_t)((L.w + 15) / 16) * ((L.h + 15) / 16);
-    w.seeds = n_seeds;
+    w.seeds = n_seeds + prior_bound(ctx->views[ref], scale);
     w.jobs = 1;
     return w;
 }
@@ -2683,6 +2790,24 @@ int seed_background(b200mvs_ctx* ctx, const std::vector<int>& lv, int n_refs, co
     return 0;
 }
 
+// The seed round's seeds are counted in an int (FrontierParams::n_seeds) and seed_key keeps a 32-bit index: a launch of the
+// entries js holds at most INT_MAX feature seeds and prior candidate bounds.  Else B200MVS_ERR_INVALID_ARG, failed_view
+// receiving the view of the last entry counted.
+int check_seed_limit(const b200mvs_ctx* ctx, const std::vector<int>& lv, const std::vector<int>& js, const int32_t* refs,
+                     const std::vector<HostPlan>& plans, int32_t* failed_view)
+{
+    uint64_t n = 0;
+    for (int j : js) {
+        n += plans[j].seeds.size() + prior_bound(ctx->views[refs[j]], lv[j]);
+        if (n > (uint64_t)INT_MAX) {
+            if (failed_view) *failed_view = refs[j];
+            return fail(B200MVS_ERR_INVALID_ARG, "a launch with view %d has %llu feature seeds and prior candidates, more than %d",
+                        refs[j], (unsigned long long)n, INT_MAX);
+        }
+    }
+    return 0;
+}
+
 // Where a reconstruction's maps go: the caller's buffers (buffer_sink) or a point set.  Right after a group's launch,
 // unless the whole group was cancelled, each view j gets its width and height in sizes[j] (when set) and, unless it was
 // cancelled, take(j, job) runs while the group's maps and pyramids are resident.  take may allocate up to bytes(w, h)
@@ -2832,13 +2957,33 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
     volatile unsigned long long* m_filled = reinterpret_cast<volatile unsigned long long*>(mirror + 1);
     volatile int* m_cancel_job = reinterpret_cast<volatile int*>(m_filled + n_refs);
     CK(cudaMemsetAsync(ctx->job_cancel.p, 0, sizeof(int) * n_refs, st));
+    // the prior seeds follow the feature seeds in run_in; the launch reads their number back once.  Their cursor is
+    // counters[C_TICKET], the ticket of k_optimize, which the frontier kernels do not use: it is zeroed again after.
+    size_t n_prior = 0;
+    if (std::any_of(js.begin(), js.end(), [&](int j) { return ctx->views[refs[j]].prior.p != nullptr; })) {
+        unsigned long long* cursor = ctx->counters.p + C_TICKET;
+        for (int k = 0; k < n_refs; ++k) {
+            const HostView& rv = ctx->views[refs[js[k]]];
+            const size_t n = prior_bound(rv, lv[js[k]]);
+            if (n == 0) continue;
+            k_prior_seeds<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(rv.prior.p, rv.prior_w, rv.prior_h, rv.prior_stride,
+                prior_cells(jobs[k].W, rv.prior_stride), n, jobs[k].W, jobs[k].H, jobs[k].conf, k, ctx->run_in.p + seeds.size(), cursor);
+            CK(cudaGetLastError());
+        }
+        unsigned long long* h_count = &ctx->h_counters->count[C_TICKET];
+        CK(cudaMemcpyAsync(h_count, cursor, sizeof(*h_count), cudaMemcpyDeviceToHost, st));
+        CK(cudaMemsetAsync(cursor, 0, sizeof(*cursor), st));
+        CK(cudaStreamSynchronize(st));
+        n_prior = (size_t)*h_count;
+        if (stats) stats->n_seeds_processed += n_prior;
+    }
 
     FrontierParams P;
     P.list[0] = ctx->ent_a.p; P.list[1] = ctx->ent_b.p;
     P.run = ctx->run_in.p; P.res = ctx->run_out.p; P.written = ctx->written.p;
     P.run2 = ctx->run_sorted.p; P.tile_cnt = ctx->tile_cnt.p; P.tile_off = ctx->tile_off.p;
     P.n_tiles = (long long)n_tiles;
-    P.cap = cap; P.n_seeds = (int)seeds.size(); P.n_jobs = n_refs;
+    P.cap = cap; P.n_seeds = (int)(seeds.size() + n_prior); P.n_jobs = n_refs;
     P.st = ctx->d_settings.p; P.jobs = ctx->d_jobs.p; P.views = ctx->d_views.p; P.lut = ctx->d_lut.p;
     P.counters = ctx->counters.p; P.ctl = ctx->ctl.p; P.hist = ctx->hist.p; P.thr_bin = ctx->thr_bin.p;
     P.host = mirror; P.host_filled = m_filled; P.host_cancel_job = m_cancel_job; P.job_cancel = ctx->job_cancel.p; P.job_run = ctx->job_run.p;
@@ -2976,6 +3121,8 @@ int reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const i
     std::vector<int> lv;
     int rc = plan_batch(ctx, s, n_refs, refs, levels, true, true, progress, failed_view, plans, lv);
     if (rc) return rc;
+    for (int j = 0; j < n_refs; ++j)
+        if ((rc = check_seed_limit(ctx, lv, {j}, refs, plans, failed_view))) return rc;
     // an image that is missing and cannot be fetched fails the call before anything runs
     if (!has_source(ctx))
         for (int j = 0; j < n_refs; ++j) {
@@ -3004,10 +3151,12 @@ int reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const i
     if (!sink && n_groups > 1)
         return fail(B200MVS_ERR_INVALID_ARG, "maps == NULL keeps the results on the device, but the budget splits the batch into %d launches", n_groups);
     ctx->mem.n_groups = (uint64_t)n_groups;
+    std::vector<std::vector<int>> group_js(n_groups);
+    for (int j = 0; j < n_refs; ++j) group_js[group_of[j]].push_back(j);
+    for (const std::vector<int>& js : group_js)
+        if ((rc = check_seed_limit(ctx, lv, js, refs, plans, failed_view))) return rc;
     std::vector<char> view_cancelled(n_refs, 0);
-    for (int g = 0; g < n_groups; ++g) {
-        std::vector<int> js;
-        for (int j = 0; j < n_refs; ++j) if (group_of[j] == g) js.push_back(j);
+    for (const std::vector<int>& js : group_js) {
         if ((rc = run_group(ctx, s, lv, js, refs, plans, seed_bg, sink, reserve, progress, stats, failed_view, view_cancelled))) return rc;
     }
     if (std::all_of(view_cancelled.begin(), view_cancelled.end(), [](char c) { return c != 0; }))

@@ -95,7 +95,7 @@ EXPORTS = ["b200mvs_default_settings", "b200mvs_create", "b200mvs_destroy", "b20
            "b200mvs_set_view_distortion", "b200mvs_set_image_source_device", "b200mvs_set_view_mask",
            "b200mvs_set_view_mask_device", "b200mvs_pset_clip_masks_device", "b200mvs_reconstruct_levels",
            "b200mvs_reconstruct_levels_device", "b200mvs_pset_add_reconstruction_levels", "b200mvs_working_set_levels",
-           "b200mvs_plan_batches_levels"]
+           "b200mvs_plan_batches_levels", "b200mvs_set_view_prior", "b200mvs_set_view_prior_device"]
 
 ERR_INVALID_ARG = -1
 ERR_CUDA = -2
@@ -210,6 +210,9 @@ def lib():
     L.b200mvs_set_view_distortion.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_float]
     L.b200mvs_set_view_mask.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int]
     L.b200mvs_set_view_mask_device.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_void_p]
+    L.b200mvs_set_view_prior.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int]
+    L.b200mvs_set_view_prior_device.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int,
+                                                C.c_void_p]
     L.b200mvs_set_view_camera.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
     L.b200mvs_num_levels.argtypes = [C.c_void_p, C.c_int]
     L.b200mvs_get_level.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -501,6 +504,49 @@ class Scene:
         stream = torch.cuda.current_stream(mask.device).cuda_stream
         self._check(self._lib.b200mvs_set_view_mask_device(self._h, view_id, C.c_void_p(mask.data_ptr()), w, h, pitch,
                                                            C.c_void_p(stream)))
+
+    def set_view_prior(self, view_id: int, depth, stride: int, on_device: bool = False):
+        """Prior depth map of a reference view (b200mvs_set_view_prior): an H x W float32 array of depths in MVE's
+        convention (distance from the camera centre along the pixel's ray, as in depth-L<s>), a numpy array or a torch
+        tensor (a CUDA tensor is copied to the host).  None clears it.  Every reconstruction then also seeds, after the
+        SfM features, the pixels x = 2 + stride i <= W - 3, y = 2 + stride k <= H - 3 of each W x H map whose prior pixel
+        ((2x+1) * prior_w // 2W, (2y+1) * prior_h // 2H) holds a finite depth > 0 and that are not masked out, so the
+        prior may have the photo's size or any level's.  The copy is kept in device memory, counted in
+        memory_stats().fixed, until the prior is cleared or replaced.
+        on_device: the prior is an H x W torch.float32 CUDA tensor on the scene's device, at any row stride, copied on the
+        device after the work of its current stream (b200mvs_set_view_prior_device), with the same results.  Anything
+        else raises ValueError."""
+        if depth is None:
+            self._check(self._lib.b200mvs_set_view_prior(self._h, view_id, None, 0, 0, 0))
+            return
+        if on_device:
+            self._set_view_prior_device(view_id, depth, stride)
+            return
+        if hasattr(depth, "detach"):                 # a torch tensor, on the host or a device
+            depth = depth.detach().cpu().numpy()
+        d = np.asarray(depth)
+        if d.ndim != 2 or d.dtype != np.float32:
+            raise ValueError("a view prior is an H x W float32 array, not %s %s" % (d.dtype, d.shape))
+        d = np.ascontiguousarray(d)
+        self._check(self._lib.b200mvs_set_view_prior(self._h, view_id, _p(d), d.shape[1], d.shape[0], int(stride)))
+
+    def _set_view_prior_device(self, view_id: int, depth, stride: int):
+        torch = _torch()
+        if (not isinstance(depth, torch.Tensor) or depth.dtype != torch.float32 or depth.dim() != 2 or not depth.is_cuda
+                or (self.device != DEVICE_NONE and depth.device != torch.device(self._torch_device()))):
+            where = "the scene's device" if self.device == DEVICE_NONE else self._torch_device()
+            raise ValueError("an on-device view prior is an H x W torch.float32 tensor on %s, not %s" % (
+                where, "%s %s on %s" % (depth.dtype, tuple(depth.shape), depth.device) if isinstance(depth, torch.Tensor)
+                else type(depth).__name__))
+        h, w = depth.shape
+        if h < 1 or w < 1:
+            raise ValueError("an on-device view prior must not be empty, not %d x %d" % (h, w))
+        if (w > 1 and depth.stride(1) != 1) or (h > 1 and depth.stride(0) < w):
+            depth = depth.contiguous()
+        pitch = 4 * (depth.stride(0) if h > 1 else w)
+        stream = torch.cuda.current_stream(depth.device).cuda_stream
+        self._check(self._lib.b200mvs_set_view_prior_device(self._h, view_id, C.c_void_p(depth.data_ptr()), w, h, pitch,
+                                                            int(stride), C.c_void_p(stream)))
 
     def set_features(self, pos: np.ndarray, refs: Sequence[np.ndarray]):
         """mve::Bundle::Features (bundle.h:51-60)."""

@@ -248,6 +248,23 @@ def silhouette(scene: Scene, v: int, width: Optional[int] = None, height: Option
     return valid.cpu().numpy().astype(np.uint8) * 255
 
 
+def depth(scene: Scene, v: int, width: Optional[int] = None, height: Optional[int] = None,
+          device: Optional[str] = None) -> np.ndarray:
+    """Analytic depth map of view v: a height x width float32 image (default: the view's size) holding, under each pixel
+    centre, the distance from the camera centre to the scene's surface along the pixel's unit ray - MVE's depth
+    convention, as in depth-L<s> - and 0 where the ray misses the surface."""
+    kind = scene.meta.get("surface") or CONFIGS[scene.name]["surface"]
+    Wv, Hv = scene.size(v)
+    w, h = width or Wv, height or Hv
+    calib = fill_calibration(scene.flen[v], scene.paspect[v], scene.ppoint[v], w, h)[0][[0, 1, 0, 1], [0, 1, 2, 2]]
+    dev = torch.device(device or "cpu")
+    pts, valid = _cast_rays(_Surface(kind, None), scene.rot[v], scene.trans[v], calib, w, h, dev)
+    R = torch.as_tensor(np.asarray(scene.rot[v]).astype(np.float64).reshape(3, 3), device=dev)
+    C = -(R.T @ torch.as_tensor(np.asarray(scene.trans[v]).astype(np.float64), device=dev))
+    d = torch.where(valid, (pts - C).norm(dim=-1), torch.zeros((), dtype=torch.float64, device=dev))
+    return d.cpu().numpy().astype(np.float32)
+
+
 def make_scene(config, device: Optional[str] = None, only_views=None, **overrides) -> Scene:
     """Build a synthetic scene. `config` is a key of CONFIGS or a dict.
     only_views: render only these views' images (the others are None) - used when ranks render their own shard.

@@ -17,6 +17,7 @@
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
+#include <cstdlib>
 #include <cstring>
 #include <ctime>
 #include <iostream>
@@ -24,6 +25,7 @@
 #include <memory>
 #include <mutex>
 #include <sstream>
+#include <string>
 #include <stdexcept>
 #include <thread>
 #include <vector>
@@ -76,6 +78,7 @@ struct DeviceCtx {
     bool features_set = false;
     bool cameras_set = false;
     std::vector<char> masks_set;    // views whose B200MVS_RECON_MASK embedding has been read
+    std::vector<char> priors_set;   // views whose B200MVS_PRIOR embedding has been read
     bool leader_active = false;
     int planners = 0;               // callers that run their global view selection right now and will enqueue next
     std::vector<Request*> pending;
@@ -185,6 +188,42 @@ void set_recon_mask(b200mvs_ctx* ctx, mve::View::Ptr view, int id, const char* e
         return;
     }
     const int rc = b200mvs_set_view_mask(ctx, id, mask->get_data_pointer(), mask->width(), mask->height());
+    if (rc != 0) throw_for(rc, b200mvs_last_error(ctx));
+}
+
+// B200MVS_PRIOR=<embedding>,<stride>: each reference view's one-channel float image of that embedding is its prior depth
+// map (b200mvs_set_view_prior), seeded every <stride> pixels; unset or empty, views grow from the features alone.  For
+// example B200MVS_PRIOR=depth-L2,4 with -s1 grows each level-1 map from the level-2 map of an earlier -s2 run as well.
+struct PriorSpec { std::string embedding; int stride = 0; };
+bool prior_spec(PriorSpec& out)
+{
+    const char* e = std::getenv("B200MVS_PRIOR");
+    if (e == nullptr || *e == '\0') return false;
+    const std::string v(e);
+    const size_t comma = v.rfind(',');
+    char* end = nullptr;
+    const long stride = comma == std::string::npos ? 0 : std::strtol(v.c_str() + comma + 1, &end, 10);
+    if (comma == std::string::npos || comma == 0 || end == v.c_str() + comma + 1 || *end != '\0' || stride < 1 || stride > 65535)
+        throw std::invalid_argument("B200MVS_PRIOR: expected <embedding>,<stride> with a stride in 1..65535, not: " + v);
+    out.embedding = v.substr(0, comma);
+    out.stride = (int)stride;
+    return true;
+}
+
+// Reads view `id`'s prior embedding into the context.  A view without it, or with one that is not a one-channel float
+// image, is reconstructed from its features alone.
+void set_prior(b200mvs_ctx* ctx, mve::View::Ptr view, int id, const PriorSpec& p)
+{
+    mve::ImageBase::Ptr img = view->get_image(p.embedding);
+    const char* problem = img == nullptr ? "Prior not found for image \"" :
+        img->get_type() != mve::IMAGE_TYPE_FLOAT || img->channels() != 1 ? "Expected 1-channel float prior for image \"" : nullptr;
+    if (problem) {
+        std::lock_guard<std::mutex> lk(g_cout);
+        std::cout << problem << view->get_name() << "\", skipping." << std::endl;
+        return;
+    }
+    const mve::FloatImage::Ptr depth = std::dynamic_pointer_cast<mve::FloatImage>(img);
+    const int rc = b200mvs_set_view_prior(ctx, id, depth->get_data_pointer(), depth->width(), depth->height(), p.stride);
     if (rc != 0) throw_for(rc, b200mvs_last_error(ctx));
 }
 
@@ -343,6 +382,7 @@ DMRecon::start()
         D.embedding = settings.imageEmbedding;
         D.held.clear();
         D.masks_set.assign(mve_views.size(), 0);
+        D.priors_set.assign(mve_views.size(), 0);
         rc = b200mvs_set_image_source(D.ctx, fetch_image, release_image, &D, device_budget());
         if (rc != 0) throw std::runtime_error(b200mvs_last_error(D.ctx));
         set_frontier_capacity(D.ctx);
@@ -431,10 +471,14 @@ DMRecon::start()
     const char* mask_embedding = recon_mask_embedding();
     const bool read_mask = mask_embedding != nullptr && !D.masks_set[req.ref];
     if (read_mask) D.masks_set[req.ref] = 1;
+    PriorSpec prior;
+    const bool read_prior = prior_spec(prior) && !D.priors_set[req.ref];
+    if (read_prior) D.priors_set[req.ref] = 1;
     D.planners++;
     lock.unlock();
     try {
         if (read_mask) set_recon_mask(ctx, mve_views[req.ref], req.ref, mask_embedding);
+        if (read_prior) set_prior(ctx, mve_views[req.ref], req.ref, prior);
     } catch (...) {
         lock.lock();
         D.planners--;
