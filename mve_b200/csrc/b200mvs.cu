@@ -683,11 +683,29 @@ std::vector<PL::SeedOut> collect_seeds(const PL::PlanInput& in, int ref, const s
     return out;
 }
 
-// The host phase of refs[j] for every j in `todo` into plans[j]: analyzeFeatures + globalViewSelection + seed list
-// (dmrecon.cc:179-292).  The per-view host work is independent (the reference runs whole DMRecons on OpenMP threads,
-// apps/dmrecon/dmrecon.cc:285): spread it over host threads.
-void make_plans(const PL::PlanInput& in, const b200mvs_settings& s, const int32_t* refs, const std::vector<int>& todo,
-                std::vector<HostPlan>& plans, b200mvs_progress* progress)
+// One entry of a batch: a reference view reconstructed at one pyramid level.  Everything below the entry points reads
+// an entry's facts from here; the batch's builder (check_batch, plan_batch) computes each of them once.
+struct BatchEntry {
+    int view = -1, level = 0;
+    HostPlan plan;
+    Workspace ws;                  // the entry's launch sizes; seeds = planned feature seeds + prior candidate bound
+    std::vector<int> need;         // the views whose pyramids it reads: itself and its global selection, ascending
+};
+
+// The entries of one call, with its settings and progress records (progress[j] belongs to e[j]; may be null)
+struct Batch {
+    b200mvs_settings s = {};
+    std::vector<BatchEntry> e;
+    b200mvs_progress* progress = nullptr;
+    int failed = -1;               // the entry whose view the call names in failed_view; -1: none
+    // the one writer of an entry point's failed_view, once the call's entries are being checked; returns rc
+    int report(int rc, int32_t* failed_view) const { if (failed_view) *failed_view = failed >= 0 ? e[failed].view : -1; return rc; }
+};
+
+// The host phase of B.e[j] for every j in `todo` into its plan: analyzeFeatures + globalViewSelection + seed list
+// (dmrecon.cc:179-292), with `s` the settings at the entries' level.  The per-view host work is independent (the
+// reference runs whole DMRecons on OpenMP threads, apps/dmrecon/dmrecon.cc:285): spread it over host threads.
+void make_plans(const PL::PlanInput& in, const b200mvs_settings& s, Batch& B, const std::vector<int>& todo)
 {
     std::atomic<size_t> next_job(0);
     auto worker = [&]() {
@@ -695,12 +713,12 @@ void make_plans(const PL::PlanInput& in, const b200mvs_settings& s, const int32_
             const size_t k = next_job.fetch_add(1);
             if (k >= todo.size()) break;
             const int j = todo[k];
-            HostPlan& p = plans[j];
+            HostPlan& p = B.e[j].plan;
             p.settings = s;
-            p.gsel = global_view_selection(in, s.min_parallax, refs[j]);
+            p.gsel = global_view_selection(in, s.min_parallax, B.e[j].view);
             if (p.gsel.empty()) continue;
-            if (progress) progress[j].status = 2;
-            p.seeds = collect_seeds(in, refs[j], p.gsel);
+            if (B.progress) B.progress[j].status = 2;
+            p.seeds = collect_seeds(in, B.e[j].view, p.gsel);
         }
     };
     const int n_threads = host_threads((int)todo.size());
@@ -2286,16 +2304,18 @@ int b200mvs_plan_views(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, 
     int rc = check_settings(s);
     if (rc) return rc;
     if (n_refs < 0 || (n_refs > 0 && !refs)) return fail(B200MVS_ERR_INVALID_ARG, "b200mvs_plan_views: bad arguments");
+    // entries at s->scale with their plans only: the workspace reads per-view state that changes under ctx->mtx
+    Batch B;
     std::vector<int> all(n_refs);
     for (int j = 0; j < n_refs; ++j) {
         if ((rc = check_ref_view(ctx, s->scale, refs[j]))) return rc;
+        B.e.push_back(BatchEntry{refs[j], s->scale});
         all[j] = j;
     }
-    std::vector<HostPlan> made(n_refs);
     std::vector<PL::PlanView> views;
-    make_plans(plan_input(ctx, *s, views), *s, refs, all, made, nullptr);
+    make_plans(plan_input(ctx, *s, views), *s, B, all);
     std::lock_guard<std::mutex> pl(ctx->plan_mtx);
-    for (int j = 0; j < n_refs; ++j) ctx->plans[refs[j]] = std::move(made[j]);
+    for (BatchEntry& E : B.e) ctx->plans[E.view] = std::move(E.plan);
     return 0;
 }
 
@@ -2389,39 +2409,36 @@ int b200mvs_optimize_patches(b200mvs_ctx* ctx, const b200mvs_settings* s, int re
 // ------------------------------------------------------------------------------------------------
 namespace {
 
-// The host phase of b200mvs_reconstruct, b200mvs_working_set and b200mvs_plan_batches: settings and per-view checks, then
-// analyzeFeatures + globalViewSelection + seed list per view (dmrecon.cc:179-292) into plans[j].  A plan prepared ahead
-// (b200mvs_plan_views, possibly while the previous batch was running) is used once and dropped when `consume`, read
-// otherwise.  A view whose selection is empty fails the call.
-// The settings and reference views of a batch (failed_view receives the view that fails).  levels: the pyramid level of
-// each entry (the *_levels entry points), or NULL for s->scale everywhere; lv receives the level of every entry.  An entry
-// is a (view, level) pair, and a call of the *_levels entry points may hold each pair once.
+// The first step of building the batch of b200mvs_reconstruct, b200mvs_working_set and b200mvs_plan_batches: the
+// settings, then the entries into B.  levels: the pyramid level of each entry (the *_levels entry points), or NULL for
+// s->scale everywhere.  An entry is a (view, level) pair, and a call of the *_levels entry points may hold each pair once.
+// B.e stays empty when the settings or the arguments fail, before any view is checked.
 int check_batch(const b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* refs, const int32_t* levels,
-                int32_t* failed_view, std::vector<int>& lv)
+                b200mvs_progress* progress, Batch& B)
 {
     int rc = check_settings(s, !levels);
     if (rc) return rc;
     if (n_refs < 1 || !refs) return fail(B200MVS_ERR_INVALID_ARG, "bad arguments");
-    lv.assign(n_refs, s->scale);
-    if (levels) lv.assign(levels, levels + n_refs);
+    B = Batch{*s, {}, progress};
+    for (int j = 0; j < n_refs; ++j) B.e.push_back(BatchEntry{refs[j], levels ? levels[j] : s->scale});
     for (int j = 0; j < n_refs; ++j) {
-        const int r = refs[j];
-        if (failed_view) *failed_view = r;
-        if ((rc = check_ref_view(ctx, lv[j], r))) return rc;
-        if (ctx->views[r].lv[lv[j]].w > 0xFFFF || ctx->views[r].lv[lv[j]].h > 0xFFFF)
-            return fail(B200MVS_ERR_UNSUPPORTED, "reference level larger than 65535 pixels per side");
+        const BatchEntry& E = B.e[j];
+        B.failed = j;
+        if ((rc = check_ref_view(ctx, E.level, E.view))) return rc;
+        const HostLevel& L = ctx->views[E.view].lv[E.level];
+        if (L.w > 0xFFFF || L.h > 0xFFFF) return fail(B200MVS_ERR_UNSUPPORTED, "reference level larger than 65535 pixels per side");
     }
+    B.failed = -1;
     if (levels) {
         std::vector<std::pair<int, int>> pairs(n_refs);
-        for (int j = 0; j < n_refs; ++j) pairs[j] = {refs[j], lv[j]};
+        for (int j = 0; j < n_refs; ++j) pairs[j] = {B.e[j].view, B.e[j].level};
         std::sort(pairs.begin(), pairs.end());
         const auto dup = std::adjacent_find(pairs.begin(), pairs.end());
         if (dup != pairs.end()) {
-            if (failed_view) *failed_view = dup->first;
+            B.failed = (int)(std::find_if(B.e.begin(), B.e.end(), [&](const BatchEntry& E) { return E.view == dup->first; }) - B.e.begin());
             return fail(B200MVS_ERR_INVALID_ARG, "view %d appears more than once at level %d", dup->first, dup->second);
         }
     }
-    if (failed_view) *failed_view = -1;
     return 0;
 }
 
@@ -2446,12 +2463,11 @@ __global__ void __launch_bounds__(PLAN_TPB) k_plan_views(const b200mvs_plan::Pla
 
 inline size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 
-// Plans refs[j] for j in `todo` on the device: one CTA per reference view, one launch per chunk of views that fits the
+// Plans B.e[j] for j in `todo` on the device: one CTA per reference view, one launch per chunk of views that fits the
 // budget next to the shared inputs.  The views it cannot plan stay in `todo` for host threads: all of them when the
 // factor table would exceed its cap (min_parallax above about 41 degrees), and any view whose workspace does not fit on
 // its own.  Every allocation goes through the accounted allocator and is freed before it returns.
-int plan_on_device(b200mvs_ctx* ctx, const b200mvs_settings& s, const PL::PlanInput& in, const int32_t* refs,
-                   std::vector<int>& todo, std::vector<HostPlan>& plans, b200mvs_progress* progress)
+int plan_on_device(b200mvs_ctx* ctx, const b200mvs_settings& s, const PL::PlanInput& in, Batch& B, std::vector<int>& todo)
 {
     const uint64_t n_table = PL::table_entries(in.dot_skip);
     if (todo.empty() || n_table == 0) return 0;
@@ -2476,7 +2492,7 @@ int plan_on_device(b200mvs_ctx* ctx, const b200mvs_settings& s, const PL::PlanIn
     struct Sized { int j; PL::PlanJob job; size_t bytes; };
     std::vector<Sized> jobs;
     for (int j : todo) {
-        const int ref = refs[j];
+        const int ref = B.e[j].view;
         PL::PlanJob J = {};
         J.ref = ref;
         J.F = in.vf_off[ref + 1] - in.vf_off[ref];
@@ -2514,7 +2530,7 @@ int plan_on_device(b200mvs_ctx* ctx, const b200mvs_settings& s, const PL::PlanIn
         d.vf_off = static_cast<const int*>(dptr[4]); d.vf_ids = static_cast<const int*>(dptr[5]);
         d.table = static_cast<const float*>(dptr[6]);
     }
-    std::vector<char> done(plans.size(), 0);
+    std::vector<char> done(B.e.size(), 0);
     b200mvs_plan_info& info = ctx->plan_info;
     size_t k0 = 0;
     while (k0 < jobs.size()) {
@@ -2553,13 +2569,13 @@ int plan_on_device(b200mvs_ctx* ctx, const b200mvs_settings& s, const PL::PlanIn
         for (size_t k = 0; k < n; ++k) {
             const uint32_t* r = &res[hj[k].out];
             const int j = jobs[k0 + k].j;
-            HostPlan& p = plans[j];
+            HostPlan& p = B.e[j].plan;
             p.settings = s;
             p.gsel.assign(reinterpret_cast<const int*>(r + PL::OUT_SEL), reinterpret_cast<const int*>(r + PL::OUT_SEL) + r[0]);
             done[j] = 1;
             info.n_device++;
             if (p.gsel.empty()) continue;
-            if (progress) progress[j].status = 2;
+            if (B.progress) B.progress[j].status = 2;
             const PL::SeedOut* so = reinterpret_cast<const PL::SeedOut*>(r + PL::OUT_HEAD);
             p.seeds.assign(so, so + r[1]);
         }
@@ -2569,113 +2585,100 @@ int plan_on_device(b200mvs_ctx* ctx, const b200mvs_settings& s, const PL::PlanIn
     return 0;
 }
 
-// `device`: the caller may plan the views that have no prepared plan on the device (plan_on_device); the inspection calls
-// and planning contexts plan on host threads.  A reconstruction's planning is recorded in ctx->plan_info.
-// levels / lv: as for check_batch.  A prepared plan serves an entry whose settings at its level are the plan's; the other
-// entries are planned once per distinct level, each with the planning input of that level, as a call at that level alone.
-int plan_batch(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* refs, const int32_t* levels, bool consume,
-               bool device, b200mvs_progress* progress, int32_t* failed_view, std::vector<HostPlan>& plans, std::vector<int>& lv)
+// The second step of building a batch: analyzeFeatures + globalViewSelection + seed list per entry (dmrecon.cc:179-292)
+// into its plan, then its workspace and needed views.  A plan prepared ahead (b200mvs_plan_views, possibly while the
+// previous batch was running) serves an entry whose settings at its level are the plan's; the other entries are planned
+// once per distinct level, each with the planning input of that level, as a call at that level alone.  A view whose
+// selection is empty fails the call.
+// `recon`: a reconstruction consumes the prepared plans it uses, may plan the others on the device (plan_on_device) and
+// records its planning in ctx->plan_info; the inspection calls read prepared plans and plan on host threads.
+int plan_batch(b200mvs_ctx* ctx, Batch& B, bool recon)
 {
-    int rc = check_batch(ctx, s, n_refs, refs, levels, failed_view, lv);
-    if (rc) return rc;
     const auto t0 = std::chrono::steady_clock::now();
-    plans.assign(n_refs, HostPlan{});
-    std::vector<int> todo;
+    const int n_refs = (int)B.e.size();
+    std::map<int, std::vector<int>> todo;            // the entries without a prepared plan, by level
     {
         const std::time_t t_start = std::time(nullptr);
         std::lock_guard<std::mutex> pl(ctx->plan_mtx);
         for (int j = 0; j < n_refs; ++j) {
-            if (progress) { progress[j].status = 1; progress[j].start_time = (uint64_t)t_start; progress[j].filled = 0; progress[j].queue_size = 0; }
-            HostPlan* p = find_plan(ctx, at_level(*s, lv[j]), refs[j]);
-            if (!p) { todo.push_back(j); continue; }
-            if (consume) { plans[j] = std::move(*p); ctx->plans.erase(refs[j]); }
-            else plans[j] = *p;
-            if (progress) progress[j].status = 2;
+            BatchEntry& E = B.e[j];
+            if (B.progress) { B.progress[j].status = 1; B.progress[j].start_time = (uint64_t)t_start; B.progress[j].filled = 0; B.progress[j].queue_size = 0; }
+            HostPlan* p = find_plan(ctx, at_level(B.s, E.level), E.view);
+            if (!p) { todo[E.level].push_back(j); continue; }
+            if (recon) { E.plan = std::move(*p); ctx->plans.erase(E.view); ctx->plan_info.n_prepared++; }
+            else E.plan = *p;
+            if (B.progress) B.progress[j].status = 2;
         }
     }
-    if (device) ctx->plan_info.n_prepared = (uint64_t)(n_refs - (int)todo.size());
-    std::vector<int> distinct(lv);
-    std::sort(distinct.begin(), distinct.end());
-    distinct.erase(std::unique(distinct.begin(), distinct.end()), distinct.end());
-    for (const int level : distinct) {
-        std::vector<int> todo_l;
-        for (int j : todo) if (lv[j] == level) todo_l.push_back(j);
-        if (todo_l.empty()) continue;
-        const b200mvs_settings sl = at_level(*s, level);
+    for (auto& [level, todo_l] : todo) {
+        const b200mvs_settings sl = at_level(B.s, level);
         std::vector<PL::PlanView> views;
         const PL::PlanInput in = plan_input(ctx, sl, views);
-        if (device) {
-            if ((rc = plan_on_device(ctx, sl, in, refs, todo_l, plans, progress))) return rc;
+        if (recon) {
+            if (int rc = plan_on_device(ctx, sl, in, B, todo_l)) return rc;
             ctx->plan_info.n_host += todo_l.size();
         }
-        make_plans(in, sl, refs, todo_l, plans, progress);
+        make_plans(in, sl, B, todo_l);
     }
-    if (device) ctx->plan_info.ms_plan = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    for (int j = 0; j < n_refs; ++j)
-        if (plans[j].gsel.empty()) { if (failed_view) *failed_view = refs[j]; return fail(B200MVS_ERR_GLOBAL_VS, "Global View Selection failed"); }
+    if (recon) ctx->plan_info.ms_plan = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    for (int j = 0; j < n_refs; ++j) {
+        BatchEntry& E = B.e[j];
+        if (E.plan.gsel.empty()) { B.failed = j; return fail(B200MVS_ERR_GLOBAL_VS, "Global View Selection failed"); }
+        const HostLevel& L = ctx->views[E.view].lv[E.level];
+        E.ws = Workspace(B.s, ctx->frontier_cap);
+        E.ws.px = (size_t)L.w * L.h;
+        E.ws.tiles = (size_t)((L.w + 15) / 16) * ((L.h + 15) / 16);
+        E.ws.seeds = E.plan.seeds.size() + prior_bound(ctx->views[E.view], E.level);
+        E.ws.jobs = 1;
+        E.need = E.plan.gsel;                    // ascending; the reference view is never selected
+        E.need.insert(std::upper_bound(E.need.begin(), E.need.end(), E.view), E.view);
+    }
     return 0;
 }
 
-// the workspace of reference view `ref` at level `scale` with n_seeds feature seeds and the candidate bound of its prior
-Workspace view_workspace(const b200mvs_ctx* ctx, const b200mvs_settings& s, int scale, int ref, size_t n_seeds)
-{
-    const HostLevel& L = ctx->views[ref].lv[scale];
-    Workspace w(s, ctx->frontier_cap);
-    w.px = (size_t)L.w * L.h;
-    w.tiles = (size_t)((L.w + 15) / 16) * ((L.h + 15) / 16);
-    w.seeds = n_seeds + prior_bound(ctx->views[ref], scale);
-    w.jobs = 1;
-    return w;
-}
-
-// the views whose pyramids the reference views refs[j], j in js, need: themselves and their global selections, ascending
-std::vector<int> views_needed(const std::vector<int>& js, const int32_t* refs, const std::vector<HostPlan>& plans)
+// the views whose pyramids the entries js need, ascending
+std::vector<int> views_of(const Batch& B, const std::vector<int>& js)
 {
     std::vector<int> v;
-    for (int j : js) { v.push_back(refs[j]); v.insert(v.end(), plans[j].gsel.begin(), plans[j].gsel.end()); }
+    for (int j : js) v.insert(v.end(), B.e[j].need.begin(), B.e[j].need.end());
     std::sort(v.begin(), v.end());
     v.erase(std::unique(v.begin(), v.end()), v.end());
     return v;
 }
 
-// lv: the level of each entry (check_batch)
-uint64_t working_set_bytes(b200mvs_ctx* ctx, const b200mvs_settings& s, const std::vector<int>& lv, const std::vector<int>& js,
-                           const int32_t* refs, const std::vector<HostPlan>& plans)
+// b200mvs_working_set of the entries js: the pyramids they need, each once, and their workspace
+uint64_t working_set_bytes(b200mvs_ctx* ctx, const Batch& B, const std::vector<int>& js)
 {
     uint64_t pyr = 0;
-    for (int v : views_needed(js, refs, plans)) pyr += pyramid_bytes(ctx->views[v]);
-    Workspace w(s, ctx->frontier_cap);
-    for (int j : js) w.add(view_workspace(ctx, s, lv[j], refs[j], plans[j].seeds.size()));
+    for (int v : views_of(B, js)) pyr += pyramid_bytes(ctx->views[v]);
+    Workspace w(B.s, ctx->frontier_cap);
+    for (int j : js) w.add(B.e[j].ws);
     return pyr + workspace_bytes(ctx, w);
 }
 
-// b200mvs_plan_batches: greedy, deterministic grouping (see the header) of the entries (refs[j] at level lv[j]).  Returns
-// the number of groups.
-int plan_groups(b200mvs_ctx* ctx, const b200mvs_settings& s, const std::vector<int>& lv, int n, const int32_t* refs,
-                const std::vector<HostPlan>& plans, uint64_t available, std::vector<int>& group_of, int32_t* failed_view)
+// b200mvs_plan_batches: greedy, deterministic grouping (see the header) of the entries of B.  Returns the number of groups.
+int plan_groups(b200mvs_ctx* ctx, Batch& B, uint64_t available, std::vector<int>& group_of)
 {
+    const int n = (int)B.e.size();
     std::vector<uint64_t> pyr_of(ctx->views.size(), 0);
     for (size_t v = 0; v < ctx->views.size(); ++v) if (ctx->views[v].valid) pyr_of[v] = pyramid_bytes(ctx->views[v]);
-    std::vector<Workspace> ws(n);
-    std::vector<std::vector<int>> need(n);
-    for (int j = 0; j < n; ++j) { ws[j] = view_workspace(ctx, s, lv[j], refs[j], plans[j].seeds.size()); need[j] = views_needed({j}, refs, plans); }
     group_of.assign(n, -1);
     std::vector<char> in_group(ctx->views.size(), 0);
     int n_groups = 0;
     for (int first = 0; first < n; ++first) {
         if (group_of[first] >= 0) continue;
         std::fill(in_group.begin(), in_group.end(), 0);
-        Workspace gw(s, ctx->frontier_cap);
+        Workspace gw(B.s, ctx->frontier_cap);
         uint64_t pyr = 0;
         int size = 0;
-        auto added = [&](int j) { uint64_t a = 0; for (int v : need[j]) if (!in_group[v]) a += pyr_of[v]; return a; };
-        auto fits = [&](int j, uint64_t a) { Workspace t = gw; t.add(ws[j]); return pyr + a + workspace_bytes(ctx, t) <= available; };
-        auto take = [&](int j, uint64_t a) { group_of[j] = n_groups; gw.add(ws[j]); pyr += a; for (int v : need[j]) in_group[v] = 1; ++size; };
+        auto added = [&](int j) { uint64_t a = 0; for (int v : B.e[j].need) if (!in_group[v]) a += pyr_of[v]; return a; };
+        auto fits = [&](int j, uint64_t a) { Workspace t = gw; t.add(B.e[j].ws); return pyr + a + workspace_bytes(ctx, t) <= available; };
+        auto take = [&](int j, uint64_t a) { group_of[j] = n_groups; gw.add(B.e[j].ws); pyr += a; for (int v : B.e[j].need) in_group[v] = 1; ++size; };
         const uint64_t a0 = added(first);
         if (!fits(first, a0)) {
-            if (failed_view) *failed_view = refs[first];
-            Workspace t = gw; t.add(ws[first]);
-            return fail(B200MVS_ERR_NO_MEMORY, "view %d needs %llu device bytes on its own, %llu are available", refs[first],
+            B.failed = first;
+            Workspace t = gw; t.add(B.e[first].ws);
+            return fail(B200MVS_ERR_NO_MEMORY, "view %d needs %llu device bytes on its own, %llu are available", B.e[first].view,
                         (unsigned long long)(a0 + workspace_bytes(ctx, t)), (unsigned long long)available);
         }
         take(first, a0);
@@ -2743,22 +2746,19 @@ int grow_frontier(b200mvs_ctx* ctx, const FrontierCtl& c, FrontierParams& P, siz
     return 0;
 }
 
-// Whether each seed of each entry lies on a background pixel of its view's reconstruction mask at the entry's level lv[j]:
-// bg[j][i] for seed i of refs[j], empty for a view without a mask.  Host masks are read on the host; the seeds of every
-// entry with a device mask are looked up by one k_seed_background launch.
-int seed_background(b200mvs_ctx* ctx, const std::vector<int>& lv, int n_refs, const int32_t* refs, const std::vector<HostPlan>& plans,
-                    std::vector<std::vector<char>>& bg)
+// Removes from each entry's seeds those on a background pixel of its view's reconstruction mask at the entry's level, in
+// place.  Host masks are read on the host; the seeds of every entry with a device mask are looked up by one
+// k_seed_background launch.  The entries' workspaces keep counting every planned seed.
+int seed_background(b200mvs_ctx* ctx, Batch& B)
 {
-    bg.assign(n_refs, {});
     std::vector<SeedMask> views;
     std::vector<int4> seeds;
-    for (int j = 0; j < n_refs; ++j) {
-        const HostView& v = ctx->views[refs[j]];
-        const HostLevel& L = v.lv[lv[j]];
-        const std::vector<PL::SeedOut>& q = plans[j].seeds;
+    for (BatchEntry& E : B.e) {
+        const HostView& v = ctx->views[E.view];
+        const HostLevel& L = v.lv[E.level];
+        std::vector<PL::SeedOut>& q = E.plan.seeds;
         if (!v.mask.empty()) {
-            bg[j].resize(q.size());
-            for (size_t i = 0; i < q.size(); ++i) bg[j][i] = background(v, L.w, L.h, q[i].x, q[i].y);
+            q.erase(std::remove_if(q.begin(), q.end(), [&](const PL::SeedOut& p) { return background(v, L.w, L.h, p.x, p.y); }), q.end());
         } else if (v.mask_dev.p && !q.empty()) {
             for (const PL::SeedOut& p : q) seeds.push_back(make_int4(p.x, p.y, (int)views.size(), 0));
             views.push_back(SeedMask{v.mask_dev.p, v.mask_w, v.mask_h, L.w, L.h});
@@ -2779,30 +2779,30 @@ int seed_background(b200mvs_ctx* ctx, const std::vector<int>& lv, int n_refs, co
     std::vector<unsigned char> flags(seeds.size());
     CK(cudaMemcpyAsync(flags.data(), d_bg.p, flags.size(), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
-    size_t at = 0;
-    for (int j = 0; j < n_refs; ++j) {
-        const HostView& v = ctx->views[refs[j]];
-        if (!v.mask.empty() || !v.mask_dev.p) continue;
-        const size_t n = plans[j].seeds.size();
-        bg[j].assign(flags.begin() + at, flags.begin() + at + n);
-        at += n;
+    const unsigned char* bg = flags.data();
+    for (BatchEntry& E : B.e) {
+        if (!ctx->views[E.view].mask_dev.p) continue;          // a view has at most one kind of mask
+        std::vector<PL::SeedOut>& q = E.plan.seeds;
+        size_t n = 0;
+        for (size_t i = 0; i < q.size(); ++i) if (!bg[i]) q[n++] = q[i];
+        bg += q.size();
+        q.resize(n);
     }
     return 0;
 }
 
 // The seed round's seeds are counted in an int (FrontierParams::n_seeds) and seed_key keeps a 32-bit index: a launch of the
-// entries js holds at most INT_MAX feature seeds and prior candidate bounds.  Else B200MVS_ERR_INVALID_ARG, failed_view
-// receiving the view of the last entry counted.
-int check_seed_limit(const b200mvs_ctx* ctx, const std::vector<int>& lv, const std::vector<int>& js, const int32_t* refs,
-                     const std::vector<HostPlan>& plans, int32_t* failed_view)
+// entries js holds at most INT_MAX feature seeds and prior candidate bounds.  Else B200MVS_ERR_INVALID_ARG, failing the
+// last entry counted.
+int check_seed_limit(Batch& B, const std::vector<int>& js)
 {
     uint64_t n = 0;
     for (int j : js) {
-        n += plans[j].seeds.size() + prior_bound(ctx->views[refs[j]], lv[j]);
+        n += B.e[j].ws.seeds;
         if (n > (uint64_t)INT_MAX) {
-            if (failed_view) *failed_view = refs[j];
+            B.failed = j;
             return fail(B200MVS_ERR_INVALID_ARG, "a launch with view %d has %llu feature seeds and prior candidates, more than %d",
-                        refs[j], (unsigned long long)n, INT_MAX);
+                        B.e[j].view, (unsigned long long)n, INT_MAX);
         }
     }
     return 0;
@@ -2819,14 +2819,13 @@ struct MapSink {
     b200mvs_maps* sizes = nullptr;
 };
 
-// One frontier launch over the entries j in js (at most MAX_GROUP_VIEWS), reference view refs[j] at level lv[j]: makes room
-// for the pyramids they need within the budget (`reserve` bytes kept free for the sink), loads the missing ones, runs, hands
-// the maps to `sink`.  Accumulates `stats`; marks the entries that ended cancelled in `view_cancelled`.  seed_bg:
-// seed_background's flags.
-int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int>& lv, const std::vector<int>& js, const int32_t* refs,
-              const std::vector<HostPlan>& plans, const std::vector<std::vector<char>>& seed_bg, const MapSink* sink, uint64_t reserve,
-              b200mvs_progress* progress, b200mvs_stats* stats, int32_t* failed_view, std::vector<char>& view_cancelled)
+// One frontier launch over the entries B.e[j], j in js (at most MAX_GROUP_VIEWS): makes room for the pyramids they need
+// within the budget (`reserve` bytes kept free for the sink), loads the missing ones, runs, hands the maps to `sink`.
+// Accumulates `stats`; marks the entries that ended cancelled in `view_cancelled`.
+int run_group(b200mvs_ctx* ctx, Batch& B, const std::vector<int>& js, const MapSink* sink, uint64_t reserve,
+              b200mvs_stats* stats, std::vector<char>& view_cancelled)
 {
+    b200mvs_progress* progress = B.progress;
     // `if (progress.cancelled) return` at the head of every stage (dmrecon.cc:100-104,336): a group whose views were all
     // cancelled before it starts loads nothing and never runs
     if (progress && std::all_of(js.begin(), js.end(), [&](int j) { return progress[j].cancelled != 0; })) {
@@ -2837,13 +2836,13 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
     const int n_refs = (int)js.size();
     cudaStream_t st = ctx->stream.get();
     std::memset(ctx->h_counters.get(), 0, sizeof(HostCounters));
-    Workspace W(*s, ctx->frontier_cap);
-    for (int j : js) W.add(view_workspace(ctx, *s, lv[j], refs[j], plans[j].seeds.size()));
+    Workspace W(B.s, ctx->frontier_cap);
+    for (int j : js) W.add(B.e[j].ws);
     WorkspaceInUse in_use(ctx);
 
     // make room: drop workspace larger than this group needs when the budget requires it, evict the pyramids the group does
     // not need (least recently used first), then load what it lacks
-    const std::vector<int> need = views_needed(js, refs, plans);
+    const std::vector<int> need = views_of(B, js);
     pin_views(ctx, need);
     uint64_t missing = 0;
     for (int v : need) if (!ctx->views[v].has_image) missing += pyramid_bytes(ctx->views[v]);
@@ -2854,10 +2853,8 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
     while (over(ws) && evict_lru(ctx)) {}
     int32_t fv = -1;
     if ((rc = load_views(ctx, need, &fv))) {
-        for (int j : js) {
-            const std::vector<int> nv = views_needed({j}, refs, plans);
-            if (std::binary_search(nv.begin(), nv.end(), (int)fv)) { if (failed_view) *failed_view = refs[j]; break; }
-        }
+        for (int j : js)
+            if (std::binary_search(B.e[j].need.begin(), B.e[j].need.end(), (int)fv)) { B.failed = j; break; }
         return rc;
     }
     if ((rc = sync_view_params(ctx))) return rc;
@@ -2868,18 +2865,15 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
     std::vector<size_t> px_off(n_refs);
     bool masked = false;                   // a view of the group has a reconstruction mask
     for (int k = 0; k < n_refs; ++k) {
-        const int j = js[k];
-        jobs[k] = make_job(ctx, lv[j], refs[j], plans[j].gsel);
+        const BatchEntry& E = B.e[js[k]];
+        jobs[k] = make_job(ctx, E.level, E.view, E.plan.gsel);
         px_off[k] = total_px;
         total_px += (size_t)jobs[k].W * jobs[k].H;
         jobs[k].tiles_x = (jobs[k].W + 15) / 16;
         jobs[k].tile_base = (long long)n_tiles;
         n_tiles += (size_t)jobs[k].tiles_x * ((jobs[k].H + 15) / 16);
-        masked = masked || ctx->views[refs[j]].masked();
-        const std::vector<char>& bg = seed_bg[j];
-        for (size_t i = 0; i < plans[j].seeds.size(); ++i) {
-            if (!bg.empty() && bg[i]) continue;
-            const PL::SeedOut& q = plans[j].seeds[i];
+        masked = masked || ctx->views[E.view].masked();
+        for (const PL::SeedOut& q : E.plan.seeds) {
             // a seed outside the image fails in the PatchSampler ctor (patch_sampler.cc:47-50); keep it so that the
             // processed count matches, the kernel rejects it by the same bounds test
             const int x = std::min(std::max(q.x, -1), 0xFFFE), y = std::min(std::max(q.y, -1), 0xFFFE);
@@ -2922,7 +2916,7 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
             unsigned char* bg_dev = reinterpret_cast<unsigned char*>(normal);
             std::vector<unsigned char> bg;
             for (int k = 0; k < n_refs; ++k) {
-                const HostView& rv = ctx->views[refs[js[k]]];
+                const HostView& rv = ctx->views[B.e[js[k]].view];
                 if (rv.mask_dev.p) {
                     const dim3 blk(32, 8), grd((jobs[k].W + 31) / 32, (jobs[k].H + 7) / 8);
                     k_mark_background<<<grd, blk, 0, st>>>(rv.mask_dev.p, rv.mask_w, rv.mask_h, jobs[k].W, jobs[k].H, bg_dev + px_off[k]);
@@ -2945,7 +2939,7 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
     CK(ctx->d_settings.reserve(1));
     CK(ctx->ctl.reserve(1));
     CK(cudaMemsetAsync(ctx->job_run.p, 0, sizeof(unsigned long long) * n_refs, st));
-    const DevSettings ds = to_dev(*s);
+    const DevSettings ds = to_dev(B.s);
     CK(cudaMemcpyAsync(ctx->d_jobs.p, jobs.data(), sizeof(JobParams) * n_refs, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(ctx->d_settings.p, &ds, sizeof(ds), cudaMemcpyHostToDevice, st));
     CK(cudaMemsetAsync(ctx->counters.p, 0, sizeof(unsigned long long) * (C_NUM + n_refs), st));
@@ -2960,11 +2954,11 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
     // the prior seeds follow the feature seeds in run_in; the launch reads their number back once.  Their cursor is
     // counters[C_TICKET], the ticket of k_optimize, which the frontier kernels do not use: it is zeroed again after.
     size_t n_prior = 0;
-    if (std::any_of(js.begin(), js.end(), [&](int j) { return ctx->views[refs[j]].prior.p != nullptr; })) {
+    if (std::any_of(js.begin(), js.end(), [&](int j) { return ctx->views[B.e[j].view].prior.p != nullptr; })) {
         unsigned long long* cursor = ctx->counters.p + C_TICKET;
         for (int k = 0; k < n_refs; ++k) {
-            const HostView& rv = ctx->views[refs[js[k]]];
-            const size_t n = prior_bound(rv, lv[js[k]]);
+            const HostView& rv = ctx->views[B.e[js[k]].view];
+            const size_t n = prior_bound(rv, B.e[js[k]].level);
             if (n == 0) continue;
             k_prior_seeds<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(rv.prior.p, rv.prior_w, rv.prior_h, rv.prior_stride,
                 prior_cells(jobs[k].W, rv.prior_stride), n, jobs[k].W, jobs[k].H, jobs[k].conf, k, ctx->run_in.p + seeds.size(), cursor);
@@ -2988,8 +2982,8 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
     P.counters = ctx->counters.p; P.ctl = ctx->ctl.p; P.hist = ctx->hist.p; P.thr_bin = ctx->thr_bin.p;
     P.host = mirror; P.host_filled = m_filled; P.host_cancel_job = m_cancel_job; P.job_cancel = ctx->job_cancel.p; P.job_run = ctx->job_run.p;
     P.thread_min = ctx->thread_min >= 0 ? ctx->thread_min : OPT_THREAD_MIN;
-    P.band_bins = s->frontier_band > 0.f ? std::max(1, (int)(s->frontier_band * (float)HIST_FINE)) : 0;
-    P.topk = (int)std::min<uint32_t>(s->frontier_topk, 1u << 30);
+    P.band_bins = B.s.frontier_band > 0.f ? std::max(1, (int)(B.s.frontier_band * (float)HIST_FINE)) : 0;
+    P.topk = (int)std::min<uint32_t>(B.s.frontier_topk, 1u << 30);
     P.first_list = 1;
 
     // views cancelled before the launch never start
@@ -3072,7 +3066,7 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
             if (sink->sizes) { sink->sizes[j].width = jobs[k].W; sink->sizes[j].height = jobs[k].H; }
             if (job_cancelled[k]) continue;                  // RECON_CANCELLED: nothing is saved (dmrecon.cc:100-104)
             if (progress) progress[j].status = 4;
-            if ((rc = sink->take(j, jobs[k]))) { if (failed_view) *failed_view = refs[j]; return rc; }
+            if ((rc = sink->take(j, jobs[k]))) { B.failed = j; return rc; }
         }
     CK(cudaStreamSynchronize(st));
     uint64_t filled = 0;
@@ -3104,49 +3098,50 @@ int run_group(b200mvs_ctx* ctx, const b200mvs_settings* s, const std::vector<int
     return 0;
 }
 
-// A reconstruction with the context locked and a device: each view's maps go to the sink after its group's launch, and no
-// group plans into the sink's bytes for the largest map of the batch; without a sink they stay on the device, one group
-// only.  levels: the level of each entry, or NULL for s->scale everywhere (check_batch).
-int reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* refs, const int32_t* levels,
-                const MapSink* sink, b200mvs_progress* progress, b200mvs_stats* stats, int32_t* failed_view)
+// The start of every reconstruction, before anything is planned: without a budget the whole batch is one launch (with
+// one, the limit applies per group), and the call's statistics, frontier and planning records start from zero.  The host
+// entry points begin before they check their entries, b200mvs_reconstruct[_levels]_device after its buffer checks.
+int begin_reconstruction(b200mvs_ctx* ctx, int n_refs, b200mvs_stats* stats)
 {
-    // without a budget the whole batch is one launch; with one, the limit applies per group
     if (!ctx->mem.budget && n_refs > MAX_GROUP_VIEWS) return fail(B200MVS_ERR_INVALID_ARG, "b200mvs_reconstruct: bad arguments");
-    if (failed_view) *failed_view = -1;
     if (stats) std::memset(stats, 0, sizeof(*stats));
     ctx->fr_initial = ctx->fr_final = ctx->fr_resumes = 0;
     ctx->plan_info = b200mvs_plan_info{};
+    return 0;
+}
+
+// The reconstruction of the checked batch B, with the context locked and a device: each entry's maps go to the sink after
+// its group's launch, and no group plans into the sink's bytes for the largest map of the batch; without a sink they stay
+// on the device, one group only.
+int run_batch(b200mvs_ctx* ctx, Batch& B, const MapSink* sink, b200mvs_stats* stats)
+{
+    const int n_refs = (int)B.e.size();
     const PinsOfCall pins(ctx);                  // each group pins the views it needs (run_group)
-    std::vector<HostPlan> plans;
-    std::vector<int> lv;
-    int rc = plan_batch(ctx, s, n_refs, refs, levels, true, true, progress, failed_view, plans, lv);
+    int rc = plan_batch(ctx, B, true);
     if (rc) return rc;
     for (int j = 0; j < n_refs; ++j)
-        if ((rc = check_seed_limit(ctx, lv, {j}, refs, plans, failed_view))) return rc;
+        if ((rc = check_seed_limit(B, {j}))) return rc;
     // an image that is missing and cannot be fetched fails the call before anything runs
     if (!has_source(ctx))
         for (int j = 0; j < n_refs; ++j) {
-            if (!ctx->views[refs[j]].has_image) { if (failed_view) *failed_view = refs[j]; return fail(B200MVS_ERR_INVALID_ARG, "color image of view %d is not loaded", refs[j]); }
-            for (int g : plans[j].gsel)
-                if (!ctx->views[g].has_image) { if (failed_view) *failed_view = refs[j]; return fail(B200MVS_ERR_INVALID_ARG, "color image of view %d (selected neighbour of view %d) is not loaded", g, refs[j]); }
+            if (!ctx->views[B.e[j].view].has_image) { B.failed = j; return fail(B200MVS_ERR_INVALID_ARG, "color image of view %d is not loaded", B.e[j].view); }
+            for (int g : B.e[j].plan.gsel)
+                if (!ctx->views[g].has_image) { B.failed = j; return fail(B200MVS_ERR_INVALID_ARG, "color image of view %d (selected neighbour of view %d) is not loaded", g, B.e[j].view); }
         }
     CK(cudaSetDevice(ctx->device));
-    std::vector<std::vector<char>> seed_bg;
-    if ((rc = seed_background(ctx, lv, n_refs, refs, plans, seed_bg))) return rc;
-    if (stats)
-        for (int j = 0; j < n_refs; ++j)
-            stats->n_seeds_processed += plans[j].seeds.size() - std::count(seed_bg[j].begin(), seed_bg[j].end(), 1);
+    if ((rc = seed_background(ctx, B))) return rc;
+    if (stats) for (const BatchEntry& E : B.e) stats->n_seeds_processed += E.plan.seeds.size();
 
     // ---- groups that fit the budget, one frontier launch each ----
     uint64_t reserve = 0;
     if (sink)
-        for (int j = 0; j < n_refs; ++j) {
-            const HostLevel& L = ctx->views[refs[j]].lv[lv[j]];
+        for (const BatchEntry& E : B.e) {
+            const HostLevel& L = ctx->views[E.view].lv[E.level];
             reserve = std::max(reserve, sink->bytes(L.w, L.h));
         }
     const uint64_t fixed = fixed_bytes(ctx), limit = budget_limit(ctx);
     std::vector<int> group_of;
-    const int n_groups = plan_groups(ctx, *s, lv, n_refs, refs, plans, limit > fixed + reserve ? limit - fixed - reserve : 0, group_of, failed_view);
+    const int n_groups = plan_groups(ctx, B, limit > fixed + reserve ? limit - fixed - reserve : 0, group_of);
     if (n_groups < 0) return n_groups;
     if (!sink && n_groups > 1)
         return fail(B200MVS_ERR_INVALID_ARG, "maps == NULL keeps the results on the device, but the budget splits the batch into %d launches", n_groups);
@@ -3154,14 +3149,26 @@ int reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const i
     std::vector<std::vector<int>> group_js(n_groups);
     for (int j = 0; j < n_refs; ++j) group_js[group_of[j]].push_back(j);
     for (const std::vector<int>& js : group_js)
-        if ((rc = check_seed_limit(ctx, lv, js, refs, plans, failed_view))) return rc;
+        if ((rc = check_seed_limit(B, js))) return rc;
     std::vector<char> view_cancelled(n_refs, 0);
     for (const std::vector<int>& js : group_js) {
-        if ((rc = run_group(ctx, s, lv, js, refs, plans, seed_bg, sink, reserve, progress, stats, failed_view, view_cancelled))) return rc;
+        if ((rc = run_group(ctx, B, js, sink, reserve, stats, view_cancelled))) return rc;
     }
     if (std::all_of(view_cancelled.begin(), view_cancelled.end(), [](char c) { return c != 0; }))
         return fail(B200MVS_ERR_CANCELLED, "reconstruction cancelled");
     return 0;
+}
+
+// A reconstruction of b200mvs_reconstruct[_levels] or b200mvs_pset_add_reconstruction[_levels], with the context locked
+// and a device.  levels: the level of each entry, or NULL for s->scale everywhere (check_batch).
+int reconstruct(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* refs, const int32_t* levels,
+                const MapSink* sink, b200mvs_progress* progress, b200mvs_stats* stats, int32_t* failed_view)
+{
+    int rc = begin_reconstruction(ctx, n_refs, stats);
+    if (rc) return rc;
+    Batch B;
+    if (!(rc = check_batch(ctx, s, n_refs, refs, levels, progress, B))) rc = run_batch(ctx, B, sink, stats);
+    return B.report(rc, failed_view);
 }
 
 // The sink into the caller's buffers `maps` (host memory, or with on_device the context's device): copies on ctx->stream,
@@ -3213,23 +3220,28 @@ int reconstruct_device(const char* fn, b200mvs_ctx* ctx, const b200mvs_settings*
 {
     std::lock_guard<std::mutex> lk(ctx->mtx);
     if (!maps_dev) return fail(B200MVS_ERR_INVALID_ARG, "%s: maps_dev is NULL", fn);
-    std::vector<int> lv;
-    int rc = check_batch(ctx, s, n_refs, refs, levels, failed_view, lv);
-    if (rc || (rc = require_device(ctx))) return rc;
-    // every buffer is checked before anything runs
-    CK(cudaSetDevice(ctx->device));
-    for (int j = 0; j < n_refs; ++j) {
-        const b200mvs_maps& m = maps_dev[j];
-        auto what = [&](const char* field) { return "maps_dev[" + std::to_string(j) + "]." + field + " (view " + std::to_string(refs[j]) + ")"; };
-        if (!m.depth) return fail(B200MVS_ERR_INVALID_ARG, "%s: %s is NULL", fn, what("depth").c_str());
-        const std::pair<const void*, const char*> bufs[] = {{m.depth, "depth"}, {m.conf, "conf"}, {m.dz, "dz"}, {m.normal, "normal"},
-                                                            {m.view_ids, "view_ids"}};
-        for (const auto& b : bufs)
-            if (b.first && (rc = check_device_buffer(fn, what(b.second), b.first, ctx->device, 4))) return rc;
-    }
-    if ((rc = wait_for_stream(ctx->ev_caller.get(), cuda_stream, ctx->stream.get()))) return rc;
-    const MapSink sink = buffer_sink(ctx, maps_dev, true);
-    return reconstruct(ctx, s, n_refs, refs, levels, &sink, progress, stats, failed_view);
+    Batch B;
+    int rc = check_batch(ctx, s, n_refs, refs, levels, progress, B);
+    if (rc && B.e.empty()) return rc;            // a settings or argument error names no view: failed_view is left as it was
+    auto run = [&]() {
+        if ((rc = require_device(ctx))) return rc;
+        // every buffer is checked before anything runs
+        CK(cudaSetDevice(ctx->device));
+        for (int j = 0; j < n_refs; ++j) {
+            const b200mvs_maps& m = maps_dev[j];
+            auto what = [&](const char* field) { return "maps_dev[" + std::to_string(j) + "]." + field + " (view " + std::to_string(refs[j]) + ")"; };
+            if (!m.depth) return fail(B200MVS_ERR_INVALID_ARG, "%s: %s is NULL", fn, what("depth").c_str());
+            const std::pair<const void*, const char*> bufs[] = {{m.depth, "depth"}, {m.conf, "conf"}, {m.dz, "dz"}, {m.normal, "normal"},
+                                                                {m.view_ids, "view_ids"}};
+            for (const auto& b : bufs)
+                if (b.first && (rc = check_device_buffer(fn, what(b.second), b.first, ctx->device, 4))) return rc;
+        }
+        if ((rc = wait_for_stream(ctx->ev_caller.get(), cuda_stream, ctx->stream.get()))) return rc;
+        if ((rc = begin_reconstruction(ctx, n_refs, stats))) return rc;
+        const MapSink sink = buffer_sink(ctx, maps_dev, true);
+        return run_batch(ctx, B, &sink, stats);
+    };
+    return B.report(rc ? rc : run(), failed_view);
 }
 
 int pset_add_reconstruction(const char* fn, b200mvs_pset* ps, b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs,
@@ -3277,13 +3289,12 @@ int pset_add_reconstruction(const char* fn, b200mvs_pset* ps, b200mvs_ctx* ctx, 
 int working_set(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const int32_t* refs, const int32_t* levels, uint64_t* bytes)
 {
     std::lock_guard<std::mutex> lk(ctx->mtx);
-    std::vector<HostPlan> plans;
-    std::vector<int> lv;
-    int rc = plan_batch(ctx, s, n_refs, refs, levels, false, false, nullptr, nullptr, plans, lv);
-    if (rc) return rc;
+    Batch B;
+    int rc = check_batch(ctx, s, n_refs, refs, levels, nullptr, B);
+    if (rc || (rc = plan_batch(ctx, B, false))) return rc;
     std::vector<int> js(n_refs);
     for (int j = 0; j < n_refs; ++j) js[j] = j;
-    *bytes = working_set_bytes(ctx, *s, lv, js, refs, plans);
+    *bytes = working_set_bytes(ctx, B, js);
     return 0;
 }
 
@@ -3291,15 +3302,12 @@ int plan_batches(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs, const 
                  uint64_t available, int32_t* group_of_ref, int32_t* failed_view)
 {
     std::lock_guard<std::mutex> lk(ctx->mtx);
-    std::vector<HostPlan> plans;
-    std::vector<int> lv;
-    int rc = plan_batch(ctx, s, n_refs, refs, levels, false, false, nullptr, failed_view, plans, lv);
-    if (rc) return rc;
+    Batch B;
     std::vector<int> group_of;
-    const int n_groups = plan_groups(ctx, *s, lv, n_refs, refs, plans, available, group_of, failed_view);
-    if (n_groups < 0) return n_groups;
-    for (int j = 0; j < n_refs; ++j) group_of_ref[j] = group_of[j];
-    return n_groups;
+    int rc = check_batch(ctx, s, n_refs, refs, levels, nullptr, B);
+    if (!rc) rc = plan_batch(ctx, B, false);
+    if (!rc && (rc = plan_groups(ctx, B, available, group_of)) > 0) std::copy(group_of.begin(), group_of.end(), group_of_ref);
+    return B.report(rc, failed_view);           // rc: the number of groups, or the error
 }
 
 } // namespace
@@ -3375,7 +3383,6 @@ int b200mvs_plan_batches(b200mvs_ctx* ctx, const b200mvs_settings* s, int n_refs
                          int32_t* group_of_ref, int32_t* failed_view)
 {
     if (!ctx || !group_of_ref) return B200MVS_ERR_INVALID_ARG;
-    if (failed_view) *failed_view = -1;
     return plan_batches(ctx, s, n_refs, refs, nullptr, available, group_of_ref, failed_view);
 }
 
