@@ -215,7 +215,7 @@ int b200mvs_set_view_mask_device(b200mvs_ctx* ctx, int view_id, const uint8_t* m
  *     pixel (floor((2x+1) w / 2W), floor((2y+1) h / 2H)), the pixel rule of b200mvs_set_view_mask, and is a seed when
  *     that value is finite and > 0 and the pixel is not background under the view's mask.
  *   - A prior seed is what a feature seed is: no local views, conf 0, the prior depth and dz 0, so the seed round runs
- *     the full local view selection for it.  Prior seeds come after every feature seed of the launch; per pixel the
+ *     the full local view selection for it (b200mvs_set_view_prior_state also carries dz and local views).  Prior seeds come after every feature seed of the launch; per pixel the
  *     most confident seed wins and the earlier one wins a tie, so a feature seed beats a prior seed of equal confidence.
  *     n_seeds_processed and n_seeds_success count the prior seeds that were made.
  *   - Every reconstruction entry point applies it: b200mvs_reconstruct[_levels][_device] and
@@ -238,6 +238,36 @@ int b200mvs_set_view_prior(b200mvs_ctx* ctx, int view_id, const float* depth_or_
  * depth_dev in host memory (pinned or pageable), on another device or not 4-byte aligned. */
 int b200mvs_set_view_prior_device(b200mvs_ctx* ctx, int view_id, const float* depth_dev_or_null, int w, int h,
                                   int64_t row_pitch, int stride, void* cuda_stream);
+/* A prior with the rest of a queue entry's state (QueueData, dmrecon.h:28-38): next to the w x h depth map, an optional
+ * w x h x 2 float dz map and an optional w x h x 4 int32 view-id map, as the dz and view_ids maps of an earlier
+ * reconstruction hold them.  b200mvs_set_view_prior(d) is this call with dz and view_ids NULL.
+ *   - Which candidates seed is the rule of b200mvs_set_view_prior, unchanged.  Candidate (x, y) of an entry with a W x H
+ *     map reads the prior pixel (px, py) of that rule.
+ *   - dz: the seed's dz is the prior's, scaled to the entry's pixel size in float32: dz_i = dz[py][px][0] * ((float)w /
+ *     (float)W) and dz_j = dz[py][px][1] * ((float)h / (float)H) (a dz is a depth change per map pixel, and one prior
+ *     pixel spans W / w map pixels).  If either is not finite, or there is no dz map, the seed's dz is (0, 0).
+ *   - Local views: the distinct ids >= 0 among the four at (px, py) that are in the entry's global view selection.  If
+ *     exactly nr_recon_neighbors (N) remain, the seed carries them as its local views, so the seed round skips the local
+ *     view selection for it, as b200mvs_optimize_patches does with n_local = N.  Otherwise, or without an id map, it
+ *     carries none and runs the full selection.  (The reference propagates 0 or N local views, never a part of a set.)
+ *   - A dz map of zeros and an id map of -1 give what no map gives: the same maps, counters and b200mvs_memory_stats
+ *     apart from the blocks' bytes.  b200mvs_working_set and b200mvs_plan_batches are unchanged: the bound is the same.
+ *   - A view has one prior.  Depth, dz and ids are copied into packed blocks of 4, 8 and 16 B per prior pixel, a block
+ *     only for a plane that is given, taken from the budget and counted in b200mvs_memory.fixed (and resident).  Any
+ *     prior call replaces every plane; one that does not fit gives B200MVS_ERR_NO_MEMORY and leaves the previous prior
+ *     whole.  NULL depth (with NULL dz and view_ids) clears the prior and frees every block.
+ *   - B200MVS_ERR_INVALID_ARG, naming the function and the field, before anything is copied: the checks of
+ *     b200mvs_set_view_prior, and dz or view_ids given with a NULL depth. */
+int b200mvs_set_view_prior_state(b200mvs_ctx* ctx, int view_id, const float* depth_or_null, const float* dz_or_null,
+                                 const int32_t* view_ids_or_null, int w, int h, int stride);
+/* The same from DEVICE memory on the context's device: row y of each plane starts at y * <plane>_pitch bytes.  Every
+ * reconstruction gives exactly what b200mvs_set_view_prior_state gives for the same values.  The stream and the return
+ * are those of b200mvs_set_view_prior_device.  Its checks, plus depth_pitch < 4 w, dz_pitch < 8 w, ids_pitch < 16 w or a
+ * given plane's pitch not a multiple of 4, and a given plane in host memory, on another device or not 4-byte aligned. */
+int b200mvs_set_view_prior_state_device(b200mvs_ctx* ctx, int view_id, const float* depth_dev_or_null,
+                                        const float* dz_dev_or_null, const int32_t* view_ids_dev_or_null, int w, int h,
+                                        int64_t depth_pitch, int64_t dz_pitch, int64_t ids_pitch, int stride,
+                                        void* cuda_stream);
 /* mve::Bundle::Features (bundle.h:51-60) as position + CSR list of referencing view ids. */
 int b200mvs_set_features(b200mvs_ctx* ctx, int n_features, const float* pos,
                          const int32_t* ref_offsets, const int32_t* ref_view_ids);

@@ -7,6 +7,7 @@
 #include "pset_device.cuh"
 #include "host_common.cuh"
 #include "plan_device.cuh"
+#include "prior_seed.cuh"
 #include "undistort.cuh"
 
 #include <algorithm>
@@ -101,14 +102,16 @@ struct HostView {
     std::vector<uint8_t> mask;     // reconstruction mask, mask_w x mask_h, 0 = background (b200mvs_set_view_mask); empty: none
     DevBuf<uint8_t> mask_dev;      // ... or the same in device memory (b200mvs_set_view_mask_device); at most one of the two
     int mask_w = 0, mask_h = 0;
-    DevBuf<float> prior;           // prior depth map, prior_w x prior_h (b200mvs_set_view_prior[_device]); null: none
+    DevBuf<float> prior;           // prior depth map, prior_w x prior_h (b200mvs_set_view_prior[_state][_device]); null: none
+    DevBuf<float2> prior_dz;       // ... its dz map (b200mvs_set_view_prior_state[_device]); null: none
+    DevBuf<int4> prior_ids;        // ... its view-id map; null: none
     int prior_w = 0, prior_h = 0, prior_stride = 0;
     float campos[3];
     float w2c[12];
     std::vector<HostLevel> lv;
     DevBuf<uchar4> pyr;            // one allocation for every level: the RGBX8 images, then their quad images
     uint64_t last_use = 0;         // eviction order: least recently used first
-    explicit HostView(b200mvs_ctx* ctx) : mask_dev(ctx), prior(ctx), pyr(ctx) {}
+    explicit HostView(b200mvs_ctx* ctx) : mask_dev(ctx), prior(ctx), prior_dz(ctx), prior_ids(ctx), pyr(ctx) {}
     bool masked() const { return !mask.empty() || mask_dev.p; }
 };
 
@@ -382,13 +385,13 @@ void release_workspace(b200mvs_ctx* ctx)
 
 // Allocations that do not depend on the batch: view table, sRGB table, settings, frontier control block and the two
 // upload staging buffers, bounded by the largest registered image at 4 channels, the device reconstruction masks and the
-// prior depth maps.
+// priors' depth, dz and view-id blocks.
 uint64_t fixed_bytes(const b200mvs_ctx* ctx)
 {
     size_t stage = 0, masks = 0;
     for (const HostView& v : ctx->views) {
         if (v.valid) stage = std::max(stage, (size_t)v.w * v.h * 4);
-        masks += v.mask_dev.bytes() + v.prior.bytes();
+        masks += v.mask_dev.bytes() + v.prior.bytes() + v.prior_dz.bytes() + v.prior_ids.bytes();
     }
     return sizeof(ViewParams) * ctx->views.size() + 256 * sizeof(float) + sizeof(DevSettings) + sizeof(FrontierCtl) + 2 * stage + masks;
 }
@@ -900,15 +903,23 @@ __global__ void k_seed_background(const SeedMask* __restrict__ views, const int4
 // k_mask_background).  Seeds are appended at out[*cursor] in whatever order the atomic gives.  That order cannot change a
 // map: every prior seed comes after the feature seeds of the launch, and the prior seeds of one entry lie on distinct
 // pixels, so the seed round's per-pixel rule (most confident first, then the earlier seed) resolves them alike in any order.
-__global__ void k_prior_seeds(const float* __restrict__ prior, int pw, int ph, int stride, int nx, size_t n, int W, int H,
-                              const float* __restrict__ conf, int job, Entry* __restrict__ out, unsigned long long* __restrict__ cursor)
+// A seed's dz and local views come from the prior's dz and id maps where they exist (prior_seed_state with the job's
+// global selection and N = nr_recon_neighbors), else it has dz 0 and no local views.
+__global__ void k_prior_seeds(const float* __restrict__ prior, const float2* __restrict__ prior_dz, const int4* __restrict__ prior_ids,
+                              int pw, int ph, int stride, int nx, size_t n, const JobParams J, unsigned N, int job,
+                              Entry* __restrict__ out, unsigned long long* __restrict__ cursor)
 {
     const size_t c = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= n) return;
     const int x = 2 + stride * (int)(c % nx), y = 2 + stride * (int)(c / nx);
-    const float d = __ldg(prior + (size_t)mask_coord(y, H, ph) * pw + mask_coord(x, W, pw));
-    if (!(d > 0.f) || isinf(d) || isinf(conf[(size_t)y * W + x])) return;
-    out[atomicAdd(cursor, 1ull)] = make_entry(pack_xy(x, y), job, 4, 0.f, d, 0.f, 0.f, 0xFFFFFFFFu);
+    const size_t q = (size_t)mask_coord(y, J.H, ph) * pw + mask_coord(x, J.W, pw);
+    const float d = __ldg(prior + q);
+    if (!(d > 0.f) || isinf(d) || isinf(J.conf[(size_t)y * J.W + x])) return;
+    PriorPixel px = {prior_dz != nullptr, prior_ids != nullptr, {0.f, 0.f}, {-1, -1, -1, -1}};
+    if (prior_dz) { const float2 t = __ldg(prior_dz + q); px.dz[0] = t.x; px.dz[1] = t.y; }
+    if (prior_ids) { const int4 t = __ldg(prior_ids + q); px.ids[0] = t.x; px.ids[1] = t.y; px.ids[2] = t.z; px.ids[3] = t.w; }
+    const PriorState s = prior_seed_state(px, pw, ph, J.W, J.H, J.gview, J.n_global, N);
+    out[atomicAdd(cursor, 1ull)] = make_entry(pack_xy(x, y), job, 4, 0.f, d, s.dzI, s.dzJ, s.slots);
 }
 // after the launch: background pixels leave the device as unfilled ones, conf = 0
 __global__ void k_unmask_background(float* __restrict__ conf, size_t n)
@@ -2078,22 +2089,39 @@ int check_prior(const char* fn, const b200mvs_ctx* ctx, int id, int w, int h, in
     return 0;
 }
 
-// Copies a w x h prior (rows `pitch` bytes apart, `kind`) into a new block of view `id`, which then replaces the old one.
-// The new block is filled before the old one goes, so a prior that does not fit leaves the previous one in place.
-int store_prior(const char* fn, b200mvs_ctx* ctx, int id, const float* src, int w, int h, size_t pitch, int stride,
-                cudaMemcpyKind kind)
+// The planes of a prior: depth, dz and view ids, with their bytes per pixel.  src[k] null: plane k is not given.
+struct PriorPlanes {
+    static constexpr size_t px_bytes[3] = {sizeof(float), sizeof(float2), sizeof(int4)};
+    const void* src[3];
+    size_t pitch[3];       // bytes from one row to the next
+};
+
+// Copies a w x h prior into new blocks of view `id`, which then replace all of its old ones: a plane that is not given
+// leaves the view without one.  The new blocks are filled before the old ones go, so a prior that does not fit leaves the
+// previous one whole.
+int store_prior(const char* fn, b200mvs_ctx* ctx, int id, const PriorPlanes& in, int w, int h, int stride, cudaMemcpyKind kind)
 {
     HostView& v = ctx->views[id];
-    DevBuf<float> block(ctx);
-    if (block.reserve((size_t)w * h) != cudaSuccess) {
+    const size_t n = (size_t)w * h;
+    DevBuf<float> depth(ctx);
+    DevBuf<float2> dz(ctx);
+    DevBuf<int4> ids(ctx);
+    if (depth.reserve(n) != cudaSuccess || (in.src[1] && dz.reserve(n) != cudaSuccess) || (in.src[2] && ids.reserve(n) != cudaSuccess)) {
         cudaGetLastError();
         return fail(B200MVS_ERR_NO_MEMORY, "%s: a %d x %d prior does not fit the device budget", fn, w, h);
     }
+    void* const dst[3] = {depth.p, dz.p, ids.p};
     cudaStream_t st = ctx->stream.get();
-    CK(cudaMemcpy2DAsync(block.p, (size_t)w * sizeof(float), src, pitch, (size_t)w * sizeof(float), (size_t)h, kind, st));
+    for (int k = 0; k < 3; ++k) {
+        if (!in.src[k]) continue;
+        const size_t row = (size_t)w * PriorPlanes::px_bytes[k];
+        CK(cudaMemcpy2DAsync(dst[k], row, in.src[k], in.pitch[k], row, (size_t)h, kind, st));
+    }
     CK(cudaStreamSynchronize(st));
-    std::swap(v.prior.p, block.p);
-    std::swap(v.prior.cap, block.cap);
+    auto take = [](auto& mine, auto& block) { std::swap(mine.p, block.p); std::swap(mine.cap, block.cap); };
+    take(v.prior, depth);
+    take(v.prior_dz, dz);
+    take(v.prior_ids, ids);
     v.prior_w = w; v.prior_h = h; v.prior_stride = stride;
     return 0;
 }
@@ -2104,39 +2132,80 @@ int clear_prior(const char* fn, b200mvs_ctx* ctx, int id)
     const int nv = (int)ctx->views.size();
     if (id < 0 || id >= nv) return fail(B200MVS_ERR_INVALID_ARG, "%s: view_id is %d, not in 0..%d", fn, id, nv - 1);
     HostView& v = ctx->views[id];
-    if (v.prior.p) { CK(cudaSetDevice(ctx->device)); v.prior.release(); }
+    if (v.prior.p) {
+        CK(cudaSetDevice(ctx->device));
+        v.prior.release();
+        v.prior_dz.release();
+        v.prior_ids.release();
+    }
     v.prior_w = v.prior_h = v.prior_stride = 0;
     return 0;
+}
+
+// Where a device prior's planes are read: their pitches, the name of the depth pitch argument and the caller's stream
+struct DevicePrior { int64_t pitch[3]; const char* depth_pitch_name; void* stream; };
+
+// The one path of the four prior calls.  dev null: the planes are packed rows in host memory.
+int set_prior(const char* fn, b200mvs_ctx* ctx, int id, const float* depth, const float* dz, const int32_t* ids, int w, int h,
+              int stride, const DevicePrior* dev)
+{
+    if (!ctx) return fail(B200MVS_ERR_INVALID_ARG, "%s: null context", fn);
+    std::lock_guard<std::mutex> lk(ctx->mtx);
+    const char* const names[3] = {dev ? "depth_dev" : "depth", dev ? "dz_dev" : "dz", dev ? "view_ids_dev" : "view_ids"};
+    PriorPlanes P = {{depth, dz, ids}, {}};
+    if (!depth) {
+        for (int k = 1; k < 3; ++k)
+            if (P.src[k]) return fail(B200MVS_ERR_INVALID_ARG, "%s: %s is given without a depth map", fn, names[k]);
+        return clear_prior(fn, ctx, id);
+    }
+    if (int rc = check_prior(fn, ctx, id, w, h, stride)) return rc;
+    for (int k = 0; k < 3; ++k) P.pitch[k] = (size_t)w * PriorPlanes::px_bytes[k];
+    if (dev) {
+        const char* const pitch_names[3] = {dev->depth_pitch_name, "dz_pitch", "ids_pitch"};
+        for (int k = 0; k < 3; ++k) {
+            const long long least = (long long)P.pitch[k], p = (long long)dev->pitch[k];
+            if (P.src[k] && (p < least || p % 4))
+                return fail(B200MVS_ERR_INVALID_ARG, "%s: %s is %lld, not a multiple of 4 of at least %d w (%lld)", fn,
+                            pitch_names[k], p, (int)PriorPlanes::px_bytes[k], least);
+            P.pitch[k] = (size_t)p;
+        }
+    }
+    CK(cudaSetDevice(ctx->device));
+    if (dev) {
+        for (int k = 0; k < 3; ++k)
+            if (P.src[k])
+                if (int rc = check_device_buffer(fn, names[k], P.src[k], ctx->device, 4)) return rc;
+        if (int rc = wait_for_stream(ctx->ev_caller.get(), dev->stream, ctx->stream.get())) return rc;
+    }
+    return store_prior(fn, ctx, id, P, w, h, stride, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice);
 }
 
 } // namespace
 
 int b200mvs_set_view_prior(b200mvs_ctx* ctx, int id, const float* depth, int w, int h, int stride)
 {
-    static const char* fn = "b200mvs_set_view_prior";
-    if (!ctx) return fail(B200MVS_ERR_INVALID_ARG, "%s: null context", fn);
-    std::lock_guard<std::mutex> lk(ctx->mtx);
-    if (!depth) return clear_prior(fn, ctx, id);
-    if (int rc = check_prior(fn, ctx, id, w, h, stride)) return rc;
-    CK(cudaSetDevice(ctx->device));
-    return store_prior(fn, ctx, id, depth, w, h, (size_t)w * sizeof(float), stride, cudaMemcpyHostToDevice);
+    return set_prior("b200mvs_set_view_prior", ctx, id, depth, nullptr, nullptr, w, h, stride, nullptr);
 }
 
 int b200mvs_set_view_prior_device(b200mvs_ctx* ctx, int id, const float* depth_dev, int w, int h, int64_t row_pitch, int stride,
                                   void* cuda_stream)
 {
-    static const char* fn = "b200mvs_set_view_prior_device";
-    if (!ctx) return fail(B200MVS_ERR_INVALID_ARG, "%s: null context", fn);
-    std::lock_guard<std::mutex> lk(ctx->mtx);
-    if (!depth_dev) return clear_prior(fn, ctx, id);
-    if (int rc = check_prior(fn, ctx, id, w, h, stride)) return rc;
-    if (row_pitch < 4ll * w || row_pitch % 4)
-        return fail(B200MVS_ERR_INVALID_ARG, "%s: row_pitch is %lld, not a multiple of 4 of at least 4 w (%lld)", fn,
-                    (long long)row_pitch, 4ll * w);
-    CK(cudaSetDevice(ctx->device));
-    if (int rc = check_device_buffer(fn, "depth_dev", depth_dev, ctx->device, 4)) return rc;
-    if (int rc = wait_for_stream(ctx->ev_caller.get(), cuda_stream, ctx->stream.get())) return rc;
-    return store_prior(fn, ctx, id, depth_dev, w, h, (size_t)row_pitch, stride, cudaMemcpyDeviceToDevice);
+    const DevicePrior dev = {{row_pitch, 0, 0}, "row_pitch", cuda_stream};
+    return set_prior("b200mvs_set_view_prior_device", ctx, id, depth_dev, nullptr, nullptr, w, h, stride, &dev);
+}
+
+int b200mvs_set_view_prior_state(b200mvs_ctx* ctx, int id, const float* depth, const float* dz, const int32_t* ids, int w,
+                                 int h, int stride)
+{
+    return set_prior("b200mvs_set_view_prior_state", ctx, id, depth, dz, ids, w, h, stride, nullptr);
+}
+
+int b200mvs_set_view_prior_state_device(b200mvs_ctx* ctx, int id, const float* depth_dev, const float* dz_dev,
+                                        const int32_t* ids_dev, int w, int h, int64_t depth_pitch, int64_t dz_pitch,
+                                        int64_t ids_pitch, int stride, void* cuda_stream)
+{
+    const DevicePrior dev = {{depth_pitch, dz_pitch, ids_pitch}, "depth_pitch", cuda_stream};
+    return set_prior("b200mvs_set_view_prior_state_device", ctx, id, depth_dev, dz_dev, ids_dev, w, h, stride, &dev);
 }
 
 int b200mvs_set_features(b200mvs_ctx* ctx, int n, const float* pos, const int32_t* off, const int32_t* ids)
@@ -2960,8 +3029,9 @@ int run_group(b200mvs_ctx* ctx, Batch& B, const std::vector<int>& js, const MapS
             const HostView& rv = ctx->views[B.e[js[k]].view];
             const size_t n = prior_bound(rv, B.e[js[k]].level);
             if (n == 0) continue;
-            k_prior_seeds<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(rv.prior.p, rv.prior_w, rv.prior_h, rv.prior_stride,
-                prior_cells(jobs[k].W, rv.prior_stride), n, jobs[k].W, jobs[k].H, jobs[k].conf, k, ctx->run_in.p + seeds.size(), cursor);
+            k_prior_seeds<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(rv.prior.p, rv.prior_dz.p, rv.prior_ids.p, rv.prior_w,
+                rv.prior_h, rv.prior_stride, prior_cells(jobs[k].W, rv.prior_stride), n, jobs[k], B.s.nr_recon_neighbors, k,
+                ctx->run_in.p + seeds.size(), cursor);
             CK(cudaGetLastError());
         }
         unsigned long long* h_count = &ctx->h_counters->count[C_TICKET];

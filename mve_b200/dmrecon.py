@@ -95,7 +95,8 @@ EXPORTS = ["b200mvs_default_settings", "b200mvs_create", "b200mvs_destroy", "b20
            "b200mvs_set_view_distortion", "b200mvs_set_image_source_device", "b200mvs_set_view_mask",
            "b200mvs_set_view_mask_device", "b200mvs_pset_clip_masks_device", "b200mvs_reconstruct_levels",
            "b200mvs_reconstruct_levels_device", "b200mvs_pset_add_reconstruction_levels", "b200mvs_working_set_levels",
-           "b200mvs_plan_batches_levels", "b200mvs_set_view_prior", "b200mvs_set_view_prior_device"]
+           "b200mvs_plan_batches_levels", "b200mvs_set_view_prior", "b200mvs_set_view_prior_device",
+           "b200mvs_set_view_prior_state", "b200mvs_set_view_prior_state_device"]
 
 ERR_INVALID_ARG = -1
 ERR_CUDA = -2
@@ -213,6 +214,10 @@ def lib():
     L.b200mvs_set_view_prior.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int]
     L.b200mvs_set_view_prior_device.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int,
                                                 C.c_void_p]
+    L.b200mvs_set_view_prior_state.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                               C.c_int]
+    L.b200mvs_set_view_prior_state_device.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                                      C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_void_p]
     L.b200mvs_set_view_camera.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
     L.b200mvs_num_levels.argtypes = [C.c_void_p, C.c_int]
     L.b200mvs_get_level.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -505,7 +510,7 @@ class Scene:
         self._check(self._lib.b200mvs_set_view_mask_device(self._h, view_id, C.c_void_p(mask.data_ptr()), w, h, pitch,
                                                            C.c_void_p(stream)))
 
-    def set_view_prior(self, view_id: int, depth, stride: int, on_device: bool = False):
+    def set_view_prior(self, view_id: int, depth, stride: int, on_device: bool = False, dz=None, view_ids=None):
         """Prior depth map of a reference view (b200mvs_set_view_prior): an H x W float32 array of depths in MVE's
         convention (distance from the camera centre along the pixel's ray, as in depth-L<s>), a numpy array or a torch
         tensor (a CUDA tensor is copied to the host).  None clears it.  Every reconstruction then also seeds, after the
@@ -515,38 +520,80 @@ class Scene:
         memory_stats().fixed, until the prior is cleared or replaced.
         on_device: the prior is an H x W torch.float32 CUDA tensor on the scene's device, at any row stride, copied on the
         device after the work of its current stream (b200mvs_set_view_prior_device), with the same results.  Anything
-        else raises ValueError."""
+        else raises ValueError.
+        dz (H x W x 2 float32) and view_ids (H x W x 4 int32), optional and of depth's H x W: the rest of each seed's
+        state (b200mvs_set_view_prior_state[_device]).  A seed's dz is the prior's, scaled to the map's pixel size, and
+        its local views are the prior's ids in the entry's global selection when there are exactly nr_recon_neighbors of
+        them, so the maps of an earlier reconstruct go straight in:
+        set_view_prior(v, m["depth"], 4, dz=m["dz"], view_ids=m["view_ids"]).  With on_device, every plane given is a
+        CUDA tensor on the scene's device."""
         if depth is None:
+            if dz is not None or view_ids is not None:
+                raise ValueError("dz and view_ids of a view prior need its depth")
             self._check(self._lib.b200mvs_set_view_prior(self._h, view_id, None, 0, 0, 0))
             return
         if on_device:
-            self._set_view_prior_device(view_id, depth, stride)
+            self._set_view_prior_device(view_id, depth, stride, dz, view_ids)
             return
-        if hasattr(depth, "detach"):                 # a torch tensor, on the host or a device
-            depth = depth.detach().cpu().numpy()
-        d = np.asarray(depth)
-        if d.ndim != 2 or d.dtype != np.float32:
-            raise ValueError("a view prior is an H x W float32 array, not %s %s" % (d.dtype, d.shape))
-        d = np.ascontiguousarray(d)
-        self._check(self._lib.b200mvs_set_view_prior(self._h, view_id, _p(d), d.shape[1], d.shape[0], int(stride)))
+        planes = []
+        for name, t, tail, dt in (("depth", depth, (), np.float32), ("dz", dz, (2,), np.float32),
+                                  ("view_ids", view_ids, (4,), np.int32)):
+            if t is None:
+                planes.append(None)
+                continue
+            if hasattr(t, "detach"):                 # a torch tensor, on the host or a device
+                t = t.detach().cpu().numpy()
+            a = np.asarray(t)
+            shape = a.shape[:2] if not planes else planes[0].shape
+            if a.ndim != 2 + len(tail) or a.shape[2:] != tail or a.shape[:2] != shape or a.dtype != dt:
+                raise ValueError("a view prior's %s is an H x W%s %s array%s, not %s %s" % (
+                    name, "".join(" x %d" % n for n in tail), np.dtype(dt).name,
+                    " of the depth's H x W %s" % (shape,) if planes else "", a.dtype, a.shape))
+            planes.append(np.ascontiguousarray(a))
+        d, z, ids = planes
+        h, w = d.shape
+        if z is None and ids is None:
+            self._check(self._lib.b200mvs_set_view_prior(self._h, view_id, _p(d), w, h, int(stride)))
+        else:
+            self._check(self._lib.b200mvs_set_view_prior_state(self._h, view_id, _p(d), None if z is None else _p(z),
+                                                               None if ids is None else _p(ids), w, h, int(stride)))
 
-    def _set_view_prior_device(self, view_id: int, depth, stride: int):
+    def _set_view_prior_device(self, view_id: int, depth, stride: int, dz=None, view_ids=None):
         torch = _torch()
-        if (not isinstance(depth, torch.Tensor) or depth.dtype != torch.float32 or depth.dim() != 2 or not depth.is_cuda
-                or (self.device != DEVICE_NONE and depth.device != torch.device(self._torch_device()))):
-            where = "the scene's device" if self.device == DEVICE_NONE else self._torch_device()
-            raise ValueError("an on-device view prior is an H x W torch.float32 tensor on %s, not %s" % (
-                where, "%s %s on %s" % (depth.dtype, tuple(depth.shape), depth.device) if isinstance(depth, torch.Tensor)
-                else type(depth).__name__))
-        h, w = depth.shape
-        if h < 1 or w < 1:
-            raise ValueError("an on-device view prior must not be empty, not %d x %d" % (h, w))
-        if (w > 1 and depth.stride(1) != 1) or (h > 1 and depth.stride(0) < w):
-            depth = depth.contiguous()
-        pitch = 4 * (depth.stride(0) if h > 1 else w)
-        stream = torch.cuda.current_stream(depth.device).cuda_stream
-        self._check(self._lib.b200mvs_set_view_prior_device(self._h, view_id, C.c_void_p(depth.data_ptr()), w, h, pitch,
-                                                            int(stride), C.c_void_p(stream)))
+        planes, pitches = [], []
+        for name, t, tail, dt in (("depth", depth, (), torch.float32), ("dz", dz, (2,), torch.float32),
+                                  ("view_ids", view_ids, (4,), torch.int32)):
+            if t is None:
+                planes.append(None)
+                pitches.append(0)
+                continue
+            shape = (tuple(t.shape[:2]) if isinstance(t, torch.Tensor) else None) if not planes else tuple(planes[0].shape)
+            if (not isinstance(t, torch.Tensor) or t.dtype != dt or t.dim() != 2 + len(tail) or not t.is_cuda
+                    or tuple(t.shape[2:]) != tail or tuple(t.shape[:2]) != shape
+                    or (self.device != DEVICE_NONE and t.device != torch.device(self._torch_device()))):
+                where = "the scene's device" if self.device == DEVICE_NONE else self._torch_device()
+                raise ValueError("an on-device view prior's %s is an H x W%s %s tensor%s on %s, not %s" % (
+                    name, "".join(" x %d" % n for n in tail), dt, " of the depth's H x W" if planes else "", where,
+                    "%s %s on %s" % (t.dtype, tuple(t.shape), t.device) if isinstance(t, torch.Tensor)
+                    else type(t).__name__))
+            h, w = t.shape[:2]
+            if h < 1 or w < 1:
+                raise ValueError("an on-device view prior must not be empty, not %d x %d" % (h, w))
+            row = w * (tail[0] if tail else 1)           # elements of a packed row
+            if not t[0].is_contiguous() or (h > 1 and t.stride(0) < row):
+                t = t.contiguous()
+            planes.append(t)
+            pitches.append(t.element_size() * (t.stride(0) if h > 1 else row))
+        d, z, ids = planes
+        h, w = d.shape
+        stream = C.c_void_p(torch.cuda.current_stream(d.device).cuda_stream)
+        ptr = [None if t is None else C.c_void_p(t.data_ptr()) for t in planes]
+        if z is None and ids is None:
+            self._check(self._lib.b200mvs_set_view_prior_device(self._h, view_id, ptr[0], w, h, pitches[0], int(stride),
+                                                                stream))
+        else:
+            self._check(self._lib.b200mvs_set_view_prior_state_device(self._h, view_id, ptr[0], ptr[1], ptr[2], w, h,
+                                                                      *pitches, int(stride), stream))
 
     def set_features(self, pos: np.ndarray, refs: Sequence[np.ndarray]):
         """mve::Bundle::Features (bundle.h:51-60)."""

@@ -194,7 +194,10 @@ void set_recon_mask(b200mvs_ctx* ctx, mve::View::Ptr view, int id, const char* e
 // B200MVS_PRIOR=<embedding>,<stride>: each reference view's one-channel float image of that embedding is its prior depth
 // map (b200mvs_set_view_prior), seeded every <stride> pixels; unset or empty, views grow from the features alone.  For
 // example B200MVS_PRIOR=depth-L2,4 with -s1 grows each level-1 map from the level-2 map of an earlier -s2 run as well.
-struct PriorSpec { std::string embedding; int stride = 0; };
+// B200MVS_PRIOR_DZ=<embedding>, read only with B200MVS_PRIOR: the view's two-channel float image of that embedding is the
+// prior's dz (b200mvs_set_view_prior_state), e.g. dz-L2 of an -s2 --keep-dz run, so each prior seed starts from the
+// coarser map's slope as well.  dmrecon saves no view ids, so a prior from its files carries depth and dz only.
+struct PriorSpec { std::string embedding, dz_embedding; int stride = 0; };
 bool prior_spec(PriorSpec& out)
 {
     const char* e = std::getenv("B200MVS_PRIOR");
@@ -207,11 +210,14 @@ bool prior_spec(PriorSpec& out)
         throw std::invalid_argument("B200MVS_PRIOR: expected <embedding>,<stride> with a stride in 1..65535, not: " + v);
     out.embedding = v.substr(0, comma);
     out.stride = (int)stride;
+    const char* dz = std::getenv("B200MVS_PRIOR_DZ");
+    out.dz_embedding = dz == nullptr ? "" : dz;
     return true;
 }
 
 // Reads view `id`'s prior embedding into the context.  A view without it, or with one that is not a one-channel float
-// image, is reconstructed from its features alone.
+// image, is reconstructed from its features alone.  A dz embedding that is missing, not a two-channel float image or of
+// another size than the depth leaves the view a depth-only prior.
 void set_prior(b200mvs_ctx* ctx, mve::View::Ptr view, int id, const PriorSpec& p)
 {
     mve::ImageBase::Ptr img = view->get_image(p.embedding);
@@ -223,7 +229,23 @@ void set_prior(b200mvs_ctx* ctx, mve::View::Ptr view, int id, const PriorSpec& p
         return;
     }
     const mve::FloatImage::Ptr depth = std::dynamic_pointer_cast<mve::FloatImage>(img);
-    const int rc = b200mvs_set_view_prior(ctx, id, depth->get_data_pointer(), depth->width(), depth->height(), p.stride);
+    const float* dz = nullptr;
+    mve::ImageBase::Ptr dz_img;
+    if (!p.dz_embedding.empty()) {
+        dz_img = view->get_image(p.dz_embedding);
+        problem = dz_img == nullptr ? "Prior dz not found for image \"" :
+            dz_img->get_type() != mve::IMAGE_TYPE_FLOAT || dz_img->channels() != 2 ? "Expected 2-channel float prior dz for image \"" :
+            dz_img->width() != depth->width() || dz_img->height() != depth->height() ? "Prior dz differs in size from the depth for image \"" :
+            nullptr;
+        if (problem) {
+            std::lock_guard<std::mutex> lk(g_cout);
+            std::cout << problem << view->get_name() << "\", using the depth alone." << std::endl;
+        } else {
+            dz = std::dynamic_pointer_cast<mve::FloatImage>(dz_img)->get_data_pointer();
+        }
+    }
+    const int rc = b200mvs_set_view_prior_state(ctx, id, depth->get_data_pointer(), dz, nullptr, depth->width(),
+                                                depth->height(), p.stride);
     if (rc != 0) throw_for(rc, b200mvs_last_error(ctx));
 }
 
