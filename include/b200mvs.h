@@ -268,6 +268,57 @@ int b200mvs_set_view_prior_state_device(b200mvs_ctx* ctx, int view_id, const flo
                                         const float* dz_dev_or_null, const int32_t* view_ids_dev_or_null, int w, int h,
                                         int64_t depth_pitch, int64_t dz_pitch, int64_t ids_pitch, int stride,
                                         void* cuda_stream);
+/* What a relative prior's values are (b200mvs_set_view_prior_relative): z is planar depth, d a value of the map. */
+enum { B200MVS_PRIOR_DISPARITY = 0,      /* 1/z = s d + t  (relative inverse-depth models)  */
+       B200MVS_PRIOR_DEPTH = 1,          /*   z = s d + t  (affine-invariant depth models)  */
+       B200MVS_PRIOR_DEPTH_SCALE = 2 };  /*   z = s d      (metric models, SfM scale unknown) */
+typedef struct b200mvs_prior_fit {
+    double   scale, shift;               /* s, t as installed (shift 0 for DEPTH_SCALE)         */
+    uint32_t n_obs, n_inliers;           /* usable feature observations, final inliers           */
+    double   median_rel_err;             /* lower median of |z_fit - z| / z over the inliers     */
+} b200mvs_prior_fit;
+/* A prior from a map known only up to a transform, such as a monocular network's disparity or depth: the view's
+ * registered features fix s and t on the device, and the map, turned into depth in MVE's convention, is installed as
+ * b200mvs_set_view_prior would install it.  values is w x h floats, row-major; kind is a B200MVS_PRIOR_* above.
+ *   - Observations: every registered feature X (b200mvs_set_features) whose refs contain the view.  Xc = R X + t with the
+ *     view's float rot and trans widened to double, z = Xc.z, which must be > 0.  u = ax Xc.x / z + cx and
+ *     v = ay Xc.y / z + cy, with ax, ay, cx, cy the float level-0 calibration of the view (fill_calibration of its
+ *     registered W0 x H0) widened to double; each expression is evaluated left to right.  The prior pixel
+ *     (floor(u w / W0), floor(v h / H0)) must lie inside the w x h map, and its value d must be finite and > 0.  The
+ *     observation is (d, y) with y = 1/z for DISPARITY and y = z for the two depth kinds.
+ *   - Fit, in double.  med is the lower median, element floor((n - 1) / 2) in ascending order, by exact selection.
+ *     Fewer than 16 observations fail.  Start: DEPTH_SCALE s = med(y/d), t = 0; the other kinds s = MAD(y) / MAD(d) and
+ *     t = med(y) - s med(d), with MAD(v) = med(|v - med v|); MAD(d) = 0 fails.  Then 3 rounds: r = y - (s d + t),
+ *     sigma = 1.4826 med(|r|) over all observations, the inliers are those with |r| <= 3 sigma (fewer than 16 fail), and
+ *     s, t are refit by least squares over them: s = sum(d y) / sum(d^2) for DEPTH_SCALE, else the centred solution
+ *     s = sum((d - dm)(y - ym)) / sum((d - dm)^2), t = ym - s dm; a zero denominator fails.  The inliers are then counted
+ *     once more with the final s and t by the same rule.  s <= 0, or s or t not finite, fails.  These constants are fixed.
+ *   - median_rel_err: z = 1/y for DISPARITY, else y; z_fit = 1/(s d + t) for DISPARITY, else s d + t.
+ *   - Apply: prior pixel (px, py) with a finite d > 0 gets z = s d + t (1/(s d + t) for DISPARITY),
+ *     a = ((px + 0.5) W0 / w - cx) / ax, b = ((py + 0.5) H0 / h - cy) / ay and depth = (float)(z sqrt(a a + b b + 1)),
+ *     each product and sum rounded on its own (no fused multiply-add).  Every other pixel, and every pixel whose z is not
+ *     finite or is <= 0, is 0.
+ *   - The depth map is installed as b200mvs_set_view_prior(view, depth, w, h, stride) installs it: the same candidates
+ *     and seeds, the same block in b200mvs_memory.fixed and resident.  It replaces any earlier prior of the view, with its
+ *     dz and ids.  A later b200mvs_set_features does not refit.
+ *   - fit_out (may be NULL) receives the fit.  A failed fit gives B200MVS_ERR_INVALID_ARG with a message that names the
+ *     function and the reason; fit_out then holds n_obs, its other fields are 0, and the view's previous prior stays.
+ *   - The observations, the fit and the apply run on the context's stream; their scratch (28 B per feature of the view,
+ *     its position and its observation, and a 64 B fit record) comes from the budget and is freed before the call returns.  A prior block or
+ *     scratch that does not fit gives B200MVS_ERR_NO_MEMORY and leaves the previous prior in place.
+ *   - B200MVS_ERR_INVALID_ARG, naming the function and the field, before anything is copied: the checks of
+ *     b200mvs_set_view_prior, a NULL values, a kind outside 0..2, a view without a camera, a context without features,
+ *     and a planning context. */
+int b200mvs_set_view_prior_relative(b200mvs_ctx* ctx, int view_id, const float* values, int w, int h, int stride,
+                                    int kind, b200mvs_prior_fit* fit_out);
+/* The same from DEVICE memory on the context's device: row y of the w x h floats starts at values_dev + y * row_pitch
+ * bytes.  It gives exactly what b200mvs_set_view_prior_relative gives for the same values: the same fit and the same
+ * prior, which the apply writes straight into the view's block.  The work runs after an event recorded on cuda_stream
+ * (NULL = the legacy default stream), and the call returns when the prior is installed.  Its checks, plus row_pitch < 4 w
+ * or not a multiple of 4, and a values_dev in host memory, on another device or not 4-byte aligned. */
+int b200mvs_set_view_prior_relative_device(b200mvs_ctx* ctx, int view_id, const float* values_dev, int w, int h,
+                                           int64_t row_pitch, int stride, int kind, void* cuda_stream,
+                                           b200mvs_prior_fit* fit_out);
 /* mve::Bundle::Features (bundle.h:51-60) as position + CSR list of referencing view ids. */
 int b200mvs_set_features(b200mvs_ctx* ctx, int n_features, const float* pos,
                          const int32_t* ref_offsets, const int32_t* ref_view_ids);

@@ -11,7 +11,7 @@ SOURCES = [os.path.join(HERE, "csrc", "b200mvs.cu"), os.path.join(HERE, "csrc", 
 DEPS = SOURCES + [os.path.join(HERE, "csrc", "patch_opt.cuh"), os.path.join(HERE, "csrc", "patch_thread.cuh"), os.path.join(HERE, "csrc", "patch_warp.cuh"),
                os.path.join(HERE, "csrc", "pset_device.cuh"), os.path.join(HERE, "csrc", "host_common.cuh"),
                os.path.join(HERE, "csrc", "plan_device.cuh"), os.path.join(HERE, "csrc", "undistort.cuh"),
-               os.path.join(HERE, "csrc", "prior_seed.cuh"),
+               os.path.join(HERE, "csrc", "prior_seed.cuh"), os.path.join(HERE, "csrc", "prior_align.cuh"),
                os.path.join(ROOT, "include", "b200mvs.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v"]

@@ -8,6 +8,7 @@
 #include "host_common.cuh"
 #include "plan_device.cuh"
 #include "prior_seed.cuh"
+#include "prior_align.cuh"
 #include "undistort.cuh"
 
 #include <algorithm>
@@ -2076,14 +2077,21 @@ int b200mvs_set_view_mask_device(b200mvs_ctx* ctx, int id, const uint8_t* mask_d
 
 namespace {
 
-// The checks of both prior calls with a prior: 0 when it may be stored
-int check_prior(const char* fn, const b200mvs_ctx* ctx, int id, int w, int h, int stride)
+// The checks of every prior call with a prior that do not depend on the context's device
+int check_prior_shape(const char* fn, const b200mvs_ctx* ctx, int id, int w, int h, int stride)
 {
     const int nv = (int)ctx->views.size();
     if (id < 0 || id >= nv) return fail(B200MVS_ERR_INVALID_ARG, "%s: view_id is %d, not in 0..%d", fn, id, nv - 1);
     if (w < 1) return fail(B200MVS_ERR_INVALID_ARG, "%s: w is %d, must be at least 1", fn, w);
     if (h < 1) return fail(B200MVS_ERR_INVALID_ARG, "%s: h is %d, must be at least 1", fn, h);
     if (stride < 1 || stride > 65535) return fail(B200MVS_ERR_INVALID_ARG, "%s: stride is %d, not in 1..65535", fn, stride);
+    return 0;
+}
+
+// The checks of both prior calls with a prior: 0 when it may be stored
+int check_prior(const char* fn, const b200mvs_ctx* ctx, int id, int w, int h, int stride)
+{
+    if (int rc = check_prior_shape(fn, ctx, id, w, h, stride)) return rc;
     if (ctx->device == B200MVS_DEVICE_NONE)
         return fail(B200MVS_ERR_INVALID_ARG, "%s: depth cannot be stored by a planning context (B200MVS_DEVICE_NONE), which has no device", fn);
     return 0;
@@ -2095,6 +2103,16 @@ struct PriorPlanes {
     const void* src[3];
     size_t pitch[3];       // bytes from one row to the next
 };
+
+// Makes filled blocks view v's prior, in place of all of its old ones (which the blocks then own and free)
+void install_prior(HostView& v, DevBuf<float>& depth, DevBuf<float2>& dz, DevBuf<int4>& ids, int w, int h, int stride)
+{
+    auto take = [](auto& mine, auto& block) { std::swap(mine.p, block.p); std::swap(mine.cap, block.cap); };
+    take(v.prior, depth);
+    take(v.prior_dz, dz);
+    take(v.prior_ids, ids);
+    v.prior_w = w; v.prior_h = h; v.prior_stride = stride;
+}
 
 // Copies a w x h prior into new blocks of view `id`, which then replace all of its old ones: a plane that is not given
 // leaves the view without one.  The new blocks are filled before the old ones go, so a prior that does not fit leaves the
@@ -2118,11 +2136,7 @@ int store_prior(const char* fn, b200mvs_ctx* ctx, int id, const PriorPlanes& in,
         CK(cudaMemcpy2DAsync(dst[k], row, in.src[k], in.pitch[k], row, (size_t)h, kind, st));
     }
     CK(cudaStreamSynchronize(st));
-    auto take = [](auto& mine, auto& block) { std::swap(mine.p, block.p); std::swap(mine.cap, block.cap); };
-    take(v.prior, depth);
-    take(v.prior_dz, dz);
-    take(v.prior_ids, ids);
-    v.prior_w = w; v.prior_h = h; v.prior_stride = stride;
+    install_prior(v, depth, dz, ids, w, h, stride);
     return 0;
 }
 
@@ -2206,6 +2220,118 @@ int b200mvs_set_view_prior_state_device(b200mvs_ctx* ctx, int id, const float* d
 {
     const DevicePrior dev = {{depth_pitch, dz_pitch, ids_pitch}, "depth_pitch", cuda_stream};
     return set_prior("b200mvs_set_view_prior_state_device", ctx, id, depth_dev, dz_dev, ids_dev, w, h, stride, &dev);
+}
+
+namespace {
+
+static_assert(B200MVS_PRIOR_DISPARITY == PRIOR_DISPARITY && B200MVS_PRIOR_DEPTH == PRIOR_DEPTH &&
+              B200MVS_PRIOR_DEPTH_SCALE == PRIOR_DEPTH_SCALE, "prior kinds of include/b200mvs.h and prior_align.cuh");
+constexpr size_t ALIGN_FIT_BYTES = 64;          // the fit record's slot in the scratch block
+static_assert(sizeof(AlignFit) <= ALIGN_FIT_BYTES, "AlignFit fits its slot");
+
+const char* align_reason(int status)
+{
+    switch (status) {
+    case ALIGN_FEW_OBS: return "fewer than 16 usable feature observations";
+    case ALIGN_FLAT: return "the map has no spread at the observations (MAD(d) = 0)";
+    case ALIGN_FEW_INLIERS: return "fewer than 16 inliers";
+    case ALIGN_SINGULAR: return "the least-squares refit is singular";
+    default: return "the scale is not positive, or the scale or shift is not finite";
+    }
+}
+
+// The one path of b200mvs_set_view_prior_relative[_device]: the observations of the view's features, the fit and the
+// apply run on the context's stream, and a fit that may be installed becomes the view's prior.  dev: values are in
+// device memory, rows `pitch` bytes apart; else packed host rows, uploaded into the new block and applied there.
+int set_prior_relative(const char* fn, b200mvs_ctx* ctx, int id, const float* values, int w, int h, int64_t pitch, int stride,
+                       int kind, bool dev, void* cuda_stream, b200mvs_prior_fit* out)
+{
+    if (!ctx) return fail(B200MVS_ERR_INVALID_ARG, "%s: null context", fn);
+    if (out) *out = b200mvs_prior_fit{};
+    std::lock_guard<std::mutex> lk(ctx->mtx);
+    const char* field = dev ? "values_dev" : "values";
+    if (int rc = check_prior_shape(fn, ctx, id, w, h, stride)) return rc;
+    if (!values) return fail(B200MVS_ERR_INVALID_ARG, "%s: %s is NULL", fn, field);
+    if (kind < B200MVS_PRIOR_DISPARITY || kind > B200MVS_PRIOR_DEPTH_SCALE)
+        return fail(B200MVS_ERR_INVALID_ARG, "%s: kind is %d, not a B200MVS_PRIOR_* kind (0..2)", fn, kind);
+    const HostView& v = ctx->views[id];
+    if (!v.valid) return fail(B200MVS_ERR_INVALID_ARG, "%s: view_id %d has no camera", fn, id);
+    if (ctx->feat_off.size() < 2) return fail(B200MVS_ERR_INVALID_ARG, "%s: the context has no features (b200mvs_set_features)", fn);
+    if (dev && (pitch < 4ll * w || pitch % 4))
+        return fail(B200MVS_ERR_INVALID_ARG, "%s: row_pitch is %lld, not a multiple of 4 of at least 4 w (%lld)", fn,
+                    (long long)pitch, 4ll * w);
+    if (ctx->device == B200MVS_DEVICE_NONE)
+        return fail(B200MVS_ERR_INVALID_ARG, "%s: %s cannot be read by a planning context (B200MVS_DEVICE_NONE), which has no device", fn, field);
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream.get();
+    if (dev) {
+        if (int rc = check_device_buffer(fn, field, values, ctx->device, 4)) return rc;
+        if (int rc = wait_for_stream(ctx->ev_caller.get(), cuda_stream, st)) return rc;
+    }
+    // the view's features, from the inverted index
+    const int* fid = ctx->vf_ids.data() + ctx->vf_off[id];
+    const unsigned m = (unsigned)(ctx->vf_off[id + 1] - ctx->vf_off[id]);
+    std::vector<float> pos(3 * (size_t)m);
+    for (unsigned i = 0; i < m; ++i) std::memcpy(&pos[3 * (size_t)i], &ctx->feat_pos[3 * (size_t)fid[i]], 3 * sizeof(float));
+    AlignCam cam;
+    for (int k = 0; k < 9; ++k) cam.R[k] = v.rot[k];
+    for (int k = 0; k < 3; ++k) cam.t[k] = v.trans[k];
+    const HostLevel& L0 = v.lv[0];
+    cam.ax = L0.proj[0]; cam.ay = L0.proj[4]; cam.cx = L0.proj[2]; cam.cy = L0.proj[5];
+    cam.W0 = v.w; cam.H0 = v.h;
+    // the new block, then the scratch: observations (16 B each), the fit record and the positions (12 B each)
+    DevBuf<float> block(ctx);
+    DevBuf<float2> no_dz(ctx);
+    DevBuf<int4> no_ids(ctx);
+    DevBuf<unsigned char> scratch(ctx);
+    const size_t obs_bytes = sizeof(double2) * (size_t)m;
+    if (block.reserve((size_t)w * h) != cudaSuccess || scratch.reserve(obs_bytes + ALIGN_FIT_BYTES + 3 * sizeof(float) * (size_t)m) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(B200MVS_ERR_NO_MEMORY, "%s: a %d x %d prior and the scratch of %u features do not fit the device budget", fn, w, h, m);
+    }
+    double2* obs = reinterpret_cast<double2*>(scratch.p);
+    AlignFit* fit = reinterpret_cast<AlignFit*>(scratch.p + obs_bytes);
+    float* pos_dev = reinterpret_cast<float*>(scratch.p + obs_bytes + ALIGN_FIT_BYTES);
+    const float* src = values;
+    size_t src_pitch = (size_t)pitch;
+    if (!dev) {
+        src_pitch = (size_t)w * sizeof(float);
+        CK(cudaMemcpyAsync(block.p, values, src_pitch * h, cudaMemcpyHostToDevice, st));
+        src = block.p;
+    }
+    if (m) {
+        CK(cudaMemcpyAsync(pos_dev, pos.data(), 3 * sizeof(float) * (size_t)m, cudaMemcpyHostToDevice, st));
+        k_align_observe<<<(m + 255) / 256, 256, 0, st>>>(pos_dev, m, cam, src, w, h, src_pitch, kind, obs);
+    }
+    k_align_fit<<<1, ALIGN_FIT_TPB, 0, st>>>(obs, m, kind, fit);
+    const dim3 blk(32, 8);
+    k_align_apply<<<dim3((w + 31) / 32, (h + 7) / 8), blk, 0, st>>>(src, src_pitch, block.p, w, h, cam, kind, fit);
+    CK(cudaGetLastError());
+    AlignFit f;
+    CK(cudaMemcpyAsync(&f, fit, sizeof(f), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (out) {
+        out->n_obs = f.n_obs;
+        if (f.status == ALIGN_OK) { out->scale = f.s; out->shift = f.t; out->n_inliers = f.n_in; out->median_rel_err = f.med_rel; }
+    }
+    if (f.status != ALIGN_OK) return fail(B200MVS_ERR_INVALID_ARG, "%s: the fit failed: %s (%u observations)", fn, align_reason(f.status), f.n_obs);
+    install_prior(ctx->views[id], block, no_dz, no_ids, w, h, stride);
+    return 0;
+}
+
+} // namespace
+
+int b200mvs_set_view_prior_relative(b200mvs_ctx* ctx, int id, const float* values, int w, int h, int stride, int kind,
+                                    b200mvs_prior_fit* fit_out)
+{
+    return set_prior_relative("b200mvs_set_view_prior_relative", ctx, id, values, w, h, 0, stride, kind, false, nullptr, fit_out);
+}
+
+int b200mvs_set_view_prior_relative_device(b200mvs_ctx* ctx, int id, const float* values_dev, int w, int h, int64_t row_pitch,
+                                           int stride, int kind, void* cuda_stream, b200mvs_prior_fit* fit_out)
+{
+    return set_prior_relative("b200mvs_set_view_prior_relative_device", ctx, id, values_dev, w, h, row_pitch, stride, kind,
+                              true, cuda_stream, fit_out);
 }
 
 int b200mvs_set_features(b200mvs_ctx* ctx, int n, const float* pos, const int32_t* off, const int32_t* ids)

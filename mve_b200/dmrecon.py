@@ -96,7 +96,8 @@ EXPORTS = ["b200mvs_default_settings", "b200mvs_create", "b200mvs_destroy", "b20
            "b200mvs_set_view_mask_device", "b200mvs_pset_clip_masks_device", "b200mvs_reconstruct_levels",
            "b200mvs_reconstruct_levels_device", "b200mvs_pset_add_reconstruction_levels", "b200mvs_working_set_levels",
            "b200mvs_plan_batches_levels", "b200mvs_set_view_prior", "b200mvs_set_view_prior_device",
-           "b200mvs_set_view_prior_state", "b200mvs_set_view_prior_state_device"]
+           "b200mvs_set_view_prior_state", "b200mvs_set_view_prior_state_device", "b200mvs_set_view_prior_relative",
+           "b200mvs_set_view_prior_relative_device"]
 
 ERR_INVALID_ARG = -1
 ERR_CUDA = -2
@@ -105,6 +106,18 @@ ERR_CANCELLED = -4
 ERR_OVERFLOW = -5
 ERR_NO_MEMORY = -7
 DEVICE_NONE = -1             # B200MVS_DEVICE_NONE: a planning context (cameras, features, view selection; no images)
+
+
+PRIOR_KINDS = {"disparity": 0, "depth": 1, "depth_scale": 2}    # B200MVS_PRIOR_* (include/b200mvs.h)
+
+
+class PriorFit(C.Structure):
+    """b200mvs_prior_fit (include/b200mvs.h)."""
+    _fields_ = [("scale", C.c_double), ("shift", C.c_double), ("n_obs", C.c_uint32), ("n_inliers", C.c_uint32),
+                ("median_rel_err", C.c_double)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
 
 
 class _Image(C.Structure):
@@ -218,6 +231,10 @@ def lib():
                                                C.c_int]
     L.b200mvs_set_view_prior_state_device.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                                       C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_void_p]
+    L.b200mvs_set_view_prior_relative.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                  C.POINTER(PriorFit)]
+    L.b200mvs_set_view_prior_relative_device.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int64,
+                                                         C.c_int, C.c_int, C.c_void_p, C.POINTER(PriorFit)]
     L.b200mvs_set_view_camera.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
     L.b200mvs_num_levels.argtypes = [C.c_void_p, C.c_int]
     L.b200mvs_get_level.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -594,6 +611,51 @@ class Scene:
         else:
             self._check(self._lib.b200mvs_set_view_prior_state_device(self._h, view_id, ptr[0], ptr[1], ptr[2], w, h,
                                                                       *pitches, int(stride), stream))
+
+    def set_view_prior_relative(self, view_id: int, values, stride: int, kind: str = "disparity") -> dict:
+        """Prior from a map known up to a transform (b200mvs_set_view_prior_relative[_device]), such as a monocular
+        network's output: kind "disparity" (1/z = s d + t), "depth" (z = s d + t) or "depth_scale" (z = s d), with z the
+        planar depth.  The view's registered features fix s and t on the device, robustly, and the map becomes a depth
+        prior in MVE's convention, installed as set_view_prior installs one.  values is an H x W float32 numpy array (the
+        host route) or a torch.float32 CUDA tensor on the scene's device at any row stride (the device route, after the
+        work of its current stream).  Returns the fit: scale, shift, n_obs, n_inliers, median_rel_err.  A failed fit
+        raises B200MVSError with the fit dict as .fit, and leaves the view's previous prior in place; a bad kind, shape,
+        dtype or device raises ValueError."""
+        if kind not in PRIOR_KINDS:
+            raise ValueError("kind is %r, not one of %s" % (kind, ", ".join(PRIOR_KINDS)))
+        fit = PriorFit()
+        if isinstance(values, np.ndarray):
+            if values.ndim != 2 or values.dtype != np.float32:
+                raise ValueError("a relative view prior is an H x W float32 array, not %s %s" % (values.dtype, values.shape))
+            v = np.ascontiguousarray(values)
+            h, w = v.shape
+            rc = self._lib.b200mvs_set_view_prior_relative(self._h, view_id, _p(v), w, h, int(stride), PRIOR_KINDS[kind],
+                                                           C.byref(fit))
+        else:
+            torch = _torch()
+            if (not isinstance(values, torch.Tensor) or values.dtype != torch.float32 or values.dim() != 2
+                    or not values.is_cuda
+                    or (self.device != DEVICE_NONE and values.device != torch.device(self._torch_device()))):
+                where = "the scene's device" if self.device == DEVICE_NONE else self._torch_device()
+                raise ValueError("a relative view prior is an H x W float32 numpy array or torch.float32 tensor on %s, "
+                                 "not %s" % (where, "%s %s on %s" % (values.dtype, tuple(values.shape), values.device)
+                                             if isinstance(values, torch.Tensor) else type(values).__name__))
+            h, w = values.shape
+            if h < 1 or w < 1:
+                raise ValueError("a relative view prior must not be empty, not %d x %d" % (h, w))
+            if not values[0].is_contiguous() or (h > 1 and values.stride(0) < w):
+                values = values.contiguous()
+            pitch = 4 * (values.stride(0) if h > 1 else w)
+            stream = torch.cuda.current_stream(values.device).cuda_stream
+            rc = self._lib.b200mvs_set_view_prior_relative_device(self._h, view_id, C.c_void_p(values.data_ptr()), w, h,
+                                                                  pitch, int(stride), PRIOR_KINDS[kind],
+                                                                  C.c_void_p(stream), C.byref(fit))
+        try:
+            self._check(rc)
+        except B200MVSError as e:
+            e.fit = fit.as_dict()
+            raise
+        return fit.as_dict()
 
     def set_features(self, pos: np.ndarray, refs: Sequence[np.ndarray]):
         """mve::Bundle::Features (bundle.h:51-60)."""

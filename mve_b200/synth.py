@@ -265,6 +265,35 @@ def depth(scene: Scene, v: int, width: Optional[int] = None, height: Optional[in
     return d.cpu().numpy().astype(np.float32)
 
 
+def monocular(scene: Scene, v: int, width: int, height: int, seed: int = 0, noise: float = 0.02,
+              outliers: float = 0.05) -> np.ndarray:
+    """A synthetic monocular prior of view v, as a relative inverse-depth network gives one: the planar disparity 1/z of
+    depth() at width x height under a seeded affine transform d = a / z + b (a in [0.5, 2], b in [0, 0.2]), with
+    multiplicative Gaussian noise of relative size `noise` and discs of random values over about `outliers` of the
+    pixels.  Where the ray misses the surface the map holds b / 2, a disparity beyond infinity, as a network's sky.
+    Float32, for Scene.set_view_prior_relative(kind="disparity")."""
+    rng = np.random.default_rng([seed, v])
+    Wv, Hv = scene.size(v)
+    K = fill_calibration(scene.flen[v], scene.paspect[v], scene.ppoint[v], Wv, Hv, np.float32)[0].astype(np.float64)
+    ray = depth(scene, v, width, height).astype(np.float64)
+    a = ((np.arange(width) + 0.5) * Wv / width - K[0, 2]) / K[0, 0]
+    b = ((np.arange(height) + 0.5) * Hv / height - K[1, 2]) / K[1, 1]
+    z = ray / np.sqrt(a[None, :] ** 2 + b[:, None] ** 2 + 1.0)
+    scale, shift = rng.uniform(0.5, 2.0), rng.uniform(0.0, 0.2)
+    with np.errstate(divide="ignore"):
+        d = np.where(z > 0, scale / np.where(z > 0, z, 1.0) + shift, shift / 2)
+    d *= 1.0 + noise * rng.standard_normal(d.shape)
+    yy, xx = np.mgrid[0:height, 0:width]
+    covered, lo, hi = np.zeros(d.shape, bool), float(d.min()), float(d.max())
+    while covered.mean() < outliers:
+        r = rng.uniform(1.0, max(2.0, 0.03 * max(width, height)))
+        cx, cy = rng.uniform(0, width), rng.uniform(0, height)
+        disc = (xx - cx) ** 2 + (yy - cy) ** 2 <= r * r
+        d[disc] = rng.uniform(lo, hi)
+        covered |= disc
+    return d.astype(np.float32)
+
+
 def make_scene(config, device: Optional[str] = None, only_views=None, **overrides) -> Scene:
     """Build a synthetic scene. `config` is a key of CONFIGS or a dict.
     only_views: render only these views' images (the others are None) - used when ranks render their own shard.

@@ -17,6 +17,7 @@
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
+#include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <ctime>
@@ -197,9 +198,35 @@ void set_recon_mask(b200mvs_ctx* ctx, mve::View::Ptr view, int id, const char* e
 // B200MVS_PRIOR_DZ=<embedding>, read only with B200MVS_PRIOR: the view's two-channel float image of that embedding is the
 // prior's dz (b200mvs_set_view_prior_state), e.g. dz-L2 of an -s2 --keep-dz run, so each prior seed starts from the
 // coarser map's slope as well.  dmrecon saves no view ids, so a prior from its files carries depth and dz only.
-struct PriorSpec { std::string embedding, dz_embedding; int stride = 0; };
+// B200MVS_PRIOR_MONO=<embedding>,<stride>,<kind>, not with B200MVS_PRIOR: the one-channel float image of that embedding
+// is a map known up to a transform, such as a monocular network's output, of kind disparity, depth or depth_scale
+// (b200mvs_set_view_prior_relative).  The view's features fix the transform, and one line per view reports it.
+struct PriorSpec { std::string embedding, dz_embedding; int stride = 0; int kind = -1; };
+bool prior_mono_spec(PriorSpec& out)
+{
+    const char* e = std::getenv("B200MVS_PRIOR_MONO");
+    if (e == nullptr || *e == '\0') return false;
+    const std::string v(e);
+    const char* p = std::getenv("B200MVS_PRIOR");
+    if (p != nullptr && *p != '\0') throw std::invalid_argument("B200MVS_PRIOR_MONO and B200MVS_PRIOR cannot both be set");
+    const size_t c1 = v.find(','), c2 = c1 == std::string::npos ? c1 : v.find(',', c1 + 1);
+    const std::string kind = c2 == std::string::npos ? "" : v.substr(c2 + 1);
+    char* end = nullptr;
+    const long stride = c2 == std::string::npos ? 0 : std::strtol(v.c_str() + c1 + 1, &end, 10);
+    out.kind = kind == "disparity" ? B200MVS_PRIOR_DISPARITY : kind == "depth" ? B200MVS_PRIOR_DEPTH :
+               kind == "depth_scale" ? B200MVS_PRIOR_DEPTH_SCALE : -1;
+    if (c2 == std::string::npos || c1 == 0 || end == v.c_str() + c1 + 1 || end != v.c_str() + c2 || stride < 1 ||
+        stride > 65535 || out.kind < 0)
+        throw std::invalid_argument("B200MVS_PRIOR_MONO: expected <embedding>,<stride>,<kind> with a stride in 1..65535 "
+                                    "and a kind of disparity, depth or depth_scale, not: " + v);
+    out.embedding = v.substr(0, c1);
+    out.stride = (int)stride;
+    return true;
+}
+
 bool prior_spec(PriorSpec& out)
 {
+    if (prior_mono_spec(out)) return true;
     const char* e = std::getenv("B200MVS_PRIOR");
     if (e == nullptr || *e == '\0') return false;
     const std::string v(e);
@@ -229,6 +256,22 @@ void set_prior(b200mvs_ctx* ctx, mve::View::Ptr view, int id, const PriorSpec& p
         return;
     }
     const mve::FloatImage::Ptr depth = std::dynamic_pointer_cast<mve::FloatImage>(img);
+    if (p.kind >= 0) {
+        b200mvs_prior_fit fit;
+        const int rc = b200mvs_set_view_prior_relative(ctx, id, depth->get_data_pointer(), depth->width(), depth->height(),
+                                                       p.stride, p.kind, &fit);
+        if (rc != 0 && rc != B200MVS_ERR_INVALID_ARG) throw_for(rc, b200mvs_last_error(ctx));
+        char line[256];
+        if (rc == 0)
+            std::snprintf(line, sizeof(line), "Prior fit for image \"%s\": s %.6g t %.6g, %u of %u inliers",
+                          view->get_name().c_str(), fit.scale, fit.shift, fit.n_inliers, fit.n_obs);
+        else   // a fit that fails leaves the view without a prior
+            std::snprintf(line, sizeof(line), "Prior fit failed for image \"%s\" (%s), skipping.", view->get_name().c_str(),
+                          b200mvs_last_error(ctx));
+        std::lock_guard<std::mutex> lk(g_cout);
+        std::cout << line << std::endl;
+        return;
+    }
     const float* dz = nullptr;
     mve::ImageBase::Ptr dz_img;
     if (!p.dz_embedding.empty()) {
